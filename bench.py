@@ -65,8 +65,10 @@ def select_model(name: str):
         UNET_TFLOP_PER_SAMPLE_EVAL, VAE_TFLOP_PER_IMAGE, VAE_ENC_TFLOP_PER_IMAGE = 6.7612, 10.4704, 4.65
         CLIP_TFLOP_PER_SEQ = 0.0133 + 0.107      # CLIP-L + OpenCLIP bigG text towers (694 M parameters x 77 tokens x 2)
         MODEL_NAME, DTYPE = "SDXL-base", "bf16"
-MUFU_EXP_PER_CLK_SM = 16      # MUFU.EX2 per clock and SM (B300_MICROARCH.md; tools/xu_probe.cu measured 4.47 T/s at 1.9 GHz)
-NUM_SMS = 148
+MUFU_EXP_PER_CLK_SM = 16      # MUFU.EX2 per clock and SM
+NUM_SMS = 132                 # H100 SXM
+MAX_SM_MHZ = 1980             # H100 SXM maximum SM clock
+DUMP_BYTES = 64_000_000       # --dump-outputs budget
 
 
 def peaks():
@@ -75,11 +77,12 @@ def peaks():
         d = json.load(open(path))
         return {"tflops_burst": d["bf16_tflops"], "tflops_sustained": d["bf16_tflops_sustained"], "hbm_gbs": d["hbm_gbs"],
                 "source": "measured"}
-    return {"tflops_burst": 1590.0, "tflops_sustained": 1400.0, "hbm_gbs": 6650.0, "source": "fallback"}
+    # NVIDIA H100 SXM data sheet (700 W): dense bf16 and HBM3 bandwidth; not a measured rate
+    return {"tflops_burst": 989.0, "tflops_sustained": 989.0, "hbm_gbs": 3350.0, "source": "H100 SXM data sheet"}
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons DURING the timed region (B200_PROFILING.md)."""
+    """nvidia-smi clocks / throttle reasons DURING the timed region."""
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,"
          "clocks_event_reasons.sw_power_cap")
@@ -240,9 +243,8 @@ def reference_http_dispatch_arm(size: str = "sd15", steps: int = STEPS_DDIM, hw:
     dispatch path: DistributedScript.before_process -> World.optimize_jobs -> Worker.request (requests.post to
     /sdapi/v1/txt2img, reference worker.py:423-448) -> postprocess_batch_list -> postprocess.  The master generates its
     share in-process while the worker's HTTP call is in flight (one thread per job, distributed.py:316-318).
-    The dispatcher is this repo's mirror of the reference's (pinned to it bit for bit by tests/test_scheduler_parity.py;
-    /root/reference itself does not travel to the GPU box — profiles/r02_reference_http_dispatch_container.json holds the
-    same run driven by the UNMODIFIED reference dispatcher in the build container); the workers are the fp32 oracle.
+    The dispatcher is this repo's mirror of the reference's (pinned to it bit for bit by tests/test_scheduler_parity.py);
+    the workers are the fp32 oracle.
     A whole request is timed for real (no extrapolation): wall clock before_process entry -> postprocess exit."""
     import logging
     import requests
@@ -428,7 +430,7 @@ def make_step(eng, workload, b, tokens_d, neg_d, x_T_d, init_d, seed0, world, ga
         lat = eng.run_program(cond, unc, pr.start(x_T_d, init), pr, CFG_SCALE, noises=draws)
         u8 = eng.decode(lat, HW, HW)
         if world > 1:
-            gather(u8, [b] * world)
+            u8 = gather(u8, [b] * world)   # the whole job's images, in global order, on every rank
         return u8
 
     return step
@@ -436,7 +438,8 @@ def make_step(eng, workload, b, tokens_d, neg_d, x_T_d, init_d, seed0, world, ga
 
 def timed_device(eng, step, steps, warmup, barrier, rank, local, world, dev):
     """W >= 3 untimed requests, then exactly K timed ones between barrier + synchronize on both sides; CUDA events, max
-    over ranks.  Returns (ms, clocks during the timed region, b200sd kernels launched inside it)."""
+    over ranks.  Returns (ms, clocks during the timed region, b200sd kernels launched inside it, what the last timed
+    request returned)."""
     import torch.distributed as dist
     from b200sd import ops
     for _ in range(max(3, warmup)):
@@ -449,8 +452,9 @@ def timed_device(eng, step, steps, warmup, barrier, rank, local, world, dev):
     barrier()
     l0 = ops.LAUNCHES + eng.graph_replayed_launches
     e0.record()
+    out = None
     for _ in range(steps):
-        step()
+        out = step()
     e1.record()
     barrier()
     launches = ops.LAUNCHES + eng.graph_replayed_launches - l0
@@ -459,7 +463,22 @@ def timed_device(eng, step, steps, warmup, barrier, rank, local, world, dev):
     t = torch.tensor([ms], device=dev)
     if world > 1:
         dist.all_reduce(t, op=dist.ReduceOp.MAX)
-    return float(t.item()), clk, launches
+    return float(t.item()), clk, launches, out
+
+
+def dump_outputs(out_dir, images):
+    """--dump-outputs: the uint8 images [B, H, W, 3] the last timed request returned -> out_dir/images.npy (float32).
+    When all of them exceed DUMP_BYTES, a fixed seeded sample of whole images is written instead; image_index.npy holds
+    the batch indices that were kept."""
+    import numpy as np
+    os.makedirs(out_dir, exist_ok=True)
+    imgs = images.detach().cpu()
+    keep = max(1, (DUMP_BYTES - 65536) // (imgs[0].numel() * 4))
+    idx = torch.arange(imgs.shape[0])
+    if imgs.shape[0] > keep:
+        idx = torch.randperm(imgs.shape[0], generator=torch.Generator().manual_seed(0))[:keep].sort().values
+    np.save(os.path.join(out_dir, "images.npy"), imgs[idx].float().numpy())
+    np.save(os.path.join(out_dir, "image_index.npy"), idx.double().numpy())
 
 
 # ================================================================================================ main
@@ -479,9 +498,13 @@ def main():
     ap.add_argument("--no-e2e", action="store_true")
     ap.add_argument("--no-world", action="store_true")
     ap.add_argument("--no-stock", action="store_true")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="after the timed steps, write the images the last timed step returned to DIR/images.npy (float32)")
     ap.add_argument("--serve-cpu-oracle", type=int, default=None, help=argparse.SUPPRESS)
     ap.add_argument("--threads", type=int, default=0, help=argparse.SUPPRESS)
     args = ap.parse_args()
+    if args.steps < 1:
+        ap.error("--steps must be at least 1")
     if args.serve_cpu_oracle is not None:
         return serve_cpu_oracle(args.serve_cpu_oracle, args.threads or usable_cpus(), args.model)
     rank, world, local = dist_env()
@@ -500,7 +523,7 @@ def main():
     config = {"workload": workload, "per_gpu_batch": args.per_gpu_batch, "global_batch": args.per_gpu_batch * world,
               "resolution": f"{px}x{px}", "sampler": SAMPLER, "timesteps": STEPS_DDIM, "unet_evals": n_evals,
               "cfg_scale": CFG_SCALE, "parallelism": f"dp{world} (batch index sharding, one all-gather at the end)",
-              "l2": "every step streams far more than the 126 MB L2 (activations of one UNet eval at batch 64 exceed 10 GB)"}
+              "l2": "every step streams far more than the 50 MB L2 (activations of one UNet eval at batch 64 exceed 10 GB)"}
 
     if args.impl == "reference":
         if rank != 0:
@@ -546,7 +569,7 @@ def main():
             tk, ng, sd0, xt, iu8 = synthetic_inputs(eng, bb, rank)
             step = make_step(eng, args.workload, bb, tk.to(dev), ng.to(dev), xt.to(dev), iu8.to(dev), sd0, world,
                              all_gather_images)
-            ms, ck, _ = timed_device(eng, step, args.steps, args.warmup, barrier, rank, local, world, dev)
+            ms, ck, _, _ = timed_device(eng, step, args.steps, args.warmup, barrier, rank, local, world, dev)
             rows.append({"per_gpu_batch": bb, "global_batch": bb * world, "value": world * bb * args.steps / (ms / 1000.0),
                          "ms_per_step": ms / args.steps, "clocks": ck})
             eng.plans.pop((bb, HW, HW), None)
@@ -571,7 +594,10 @@ def main():
     tokens, neg, seed0, x_T, init_u8 = synthetic_inputs(eng, b, rank)
     step_device = make_step(eng, args.workload, b, tokens.to(dev), neg.to(dev), x_T.to(dev), init_u8.to(dev), seed0, world,
                             all_gather_images)
-    elapsed_ms, clk, gpu_launches = timed_device(eng, step_device, args.steps, args.warmup, barrier, rank, local, world, dev)
+    elapsed_ms, clk, gpu_launches, last = timed_device(eng, step_device, args.steps, args.warmup, barrier, rank, local, world,
+                                                       dev)
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, last)   # with N GPUs: the all-gathered images of the whole job
     value = world * b * args.steps / (elapsed_ms / 1000.0)
 
     # ---------------- e2e through the plugin surface (host buffers, H2D + D2H inside the timed region), one world per rank
@@ -771,8 +797,9 @@ def kernel_rooflines(eng, b, pk, clk):
                       "conv2d": {"ms": tc[1][1], "tflops": tc[1][2] / max(tc[1][1], 1e-9) / 1e9}},
             "peak_source": pk["source"] + " sustained bf16 cuBLAS"}
     at = agg.get("attention", [0, 1e-9, 0])
-    sm_mhz = (clk or {}).get("sm_mhz") or 1965.0
+    sm_mhz = (clk or {}).get("sm_mhz") or float(MAX_SM_MHZ)
     exp_peak_run = NUM_SMS * MUFU_EXP_PER_CLK_SM * sm_mhz * 1e6 / 1e12
+    exp_peak_boost = NUM_SMS * MUFU_EXP_PER_CLK_SM * MAX_SM_MHZ * 1e6 / 1e12
     exp_ach = exps[0] / (at[1] * 1e-3) / 1e12
     roof_attn = {"kernel": "attention_tc_kernel", "bound": "tensor", "achieved": at[2] / (at[1] * 1e-3) / 1e12, "peak": peak,
                  "unit": "TFLOP/s", "frac": at[2] / (at[1] * 1e-3) / 1e12 / peak, "launches": at[0], "ms": at[1],
@@ -780,9 +807,9 @@ def kernel_rooflines(eng, b, pk, clk):
                  # the pipe that actually bounds it: one MUFU.EX2 per S element, 16 per clock and SM
                  "exp_rate": {"achieved": exp_ach, "unit": "T exp/s",
                               "peak_at_run_clock": exp_peak_run, "frac_at_run_clock": exp_ach / exp_peak_run,
-                              "peak_at_boost": 4.47, "frac_at_boost": exp_ach / 4.47,
-                              "peak_source": f"148 SMs x 16 MUFU.EX2/clk x {sm_mhz:.0f} MHz (median SM clock of the timed region); "
-                                             "4.47 measured by tools/xu_probe.cu at boost"}}
+                              "peak_at_boost": exp_peak_boost, "frac_at_boost": exp_ach / exp_peak_boost,
+                              "peak_source": f"{NUM_SMS} SMs x 16 MUFU.EX2/clk x {sm_mhz:.0f} MHz (median SM clock of the timed "
+                                             f"region); at boost: x {MAX_SM_MHZ} MHz"}}
     breakdown = {k: round(v[1], 3) for k, v in agg.items()}
     # HBM-bound kernel classes: algorithmic bytes (DESIGN.md section 4: GroupNorm 2 reads + 1 write of 45.1 M elements per
     # sample-evaluation, LayerNorm 1 read + 1 write of 34.7 M) over the summed CUDA-event durations, against the measured

@@ -1,4 +1,4 @@
-/* b200sd.h — C ABI of libb200sd.so, the sm_100a compute library behind the local-GPU worker.
+/* b200sd.h — C ABI of libb200sd.so, the sm_90a (H100) compute library behind the local-GPU worker.
  *
  * Boundary being replaced (reference = papuSpartan/stable-diffusion-webui-distributed @ 8fd65ebd):
  *   scripts/spartan/worker.py:288-504  Worker.request()  — the reference posts the job to a remote sdwui
@@ -45,15 +45,14 @@ typedef struct b200sd_epilogue {
   int flags;              /* B200SD_EPI_* */
 } b200sd_epilogue;
 
-/* library / build identification: returns a static string "b200sd <version> sm_100a" */
+/* library / build identification: returns a static string "b200sd <version> sm_90a" */
 const char* b200sd_version(void);
-/* debug: a device buffer of 16 x 64 int64 that one CTA of every later b200sd_attention launch fills with clock64()
- * stamps of its per-tile pipeline events (tools/attn_trace.py); NULL switches it off (default). */
+/* debug hooks kept for ABI compatibility: the sm_90a attention and GEMM / conv kernels record no timeline, so the buffer is
+ * never written; both return 0. */
 int b200sd_debug_attention_trace(void* device_buffer);
-/* debug only: clock64 timeline of CTA 0 of the GEMM / conv kernel (tools/gemm_trace.py; trace-enabled builds). */
 int b200sd_debug_gemm_trace(void* device_buffer);
 
-/* ---- tensor-core ops (tcgen05 + TMA) ----------------------------------------------------------- */
+/* ---- tensor-core ops (wgmma + TMA) -------------------------------------------------------------- */
 
 /* D[M,N_out] = epi(A[M,K] . Wt[N,K]^T).  Linear layers and 1x1 convs (upstream ldm CrossAttention.to_q/k/v/
  * to_out, FeedForward.net, SpatialTransformer.proj_in/out, ResBlock.skip_connection).
@@ -95,15 +94,15 @@ int b200sd_groupnorm_apply(const void* X, long long pitch_x, void* Y, long long 
  * keeps its ~48 KB slab of an image in shared memory while the image's CTAs agree on the statistics (1 read + 1 write
  * instead of 2 reads + 1 write) — or B200SD_ERR_UNSUPPORTED when the shape is not eligible (C <= 2048, G <= 64 and all
  * slabs of ONE image resident on the device at the same time: a function of HW and C only, never of NB, so an image's bits
- * do not depend on the batch it travels in).  mode 0: mode 1, unless B200SD_GN_FUSED=1 and the shape is eligible (measured
- * on B200 the one-pass kernel is the slower one at the UNet's shapes: the cross-CTA agreement costs more than the second
- * read it saves, DESIGN.md section 4).  `stats` as for b200sd_groupnorm_stats. */
+ * do not depend on the batch it travels in).  mode 0: mode 1, unless B200SD_GN_FUSED=1 and the shape is eligible (the
+ * cross-CTA agreement of the one-pass kernel can cost more than the second read it saves, DESIGN.md section 4).  `stats` as
+ * for b200sd_groupnorm_stats. */
 int b200sd_groupnorm(const void* X, long long pitch_x, void* Y, long long pitch_y, int NB, int HW, int C, int G,
                      float* stats, const float* gamma, const float* beta, float eps, int silu, int mode, int dtype,
                      void* stream);
 /* 1 if modes 0 / 2 take the one-pass kernel for this shape on the current device. */
 int b200sd_groupnorm_is_fused(int NB, int HW, int C, int G, int dtype);
-/* measurement aid (tools/norm_sweep.py): slab KB of the one-pass kernel, 8..160 (0 = keep; default 48, env
+/* measurement aid: slab KB of the one-pass kernel, 8..160 (0 = keep; default 48, env
  * B200SD_GN_FUSED_KB) — call b200sd_groupnorm_stats_floats again afterwards — and whether the statistics kernel walks the
  * tensor back to front (-1 = keep; default 1, env B200SD_GN_REVERSE). */
 int b200sd_debug_gn_config(int slab_kb, int reverse_stats);

@@ -44,7 +44,7 @@ def declared_symbols(header: str = HEADER_PATH):
 def load(path: str = LIB_PATH) -> ctypes.CDLL:
     if not os.path.exists(path):
         raise B200SDError(
-            f"{path} not found: build it with `python __graft_entry__.py` (nvcc, sm_100a). "
+            f"{path} not found: build it with `python __graft_entry__.py` (nvcc, sm_90a). "
             "There is no CPU or PyTorch fallback for the hot path.")
     lib = ctypes.CDLL(path)
     for name in declared_symbols():

@@ -1,108 +1,56 @@
-// attention_tc.cu — flash-attention forward (non-causal) on tcgen05 for sm_100a.
+// attention_tc.cu — flash-attention forward (non-causal) on wgmma for sm_90a.
 //
 //   O[b, s, h, :] = softmax(Q[b, s, h, :] . K[b, :, h, :]^T * scale) . V[b, :, h, :]
 //
 // Covers the UNet's self-attention (S = 4096/1024/256/64, d = 40/80/160) and cross-attention (77 context
-// tokens) — upstream ldm CrossAttention (SURVEY.md §8 a-ext x6, x7; not in /root/reference).
+// tokens) — upstream ldm CrossAttention (SURVEY.md §8 a-ext x6, x7).
 //
-// Layout: Q/K/V rows are tokens; every head owns d_pad (multiple of 64) consecutive halfs, the first d of
-// which are data and the rest zero (the projection GEMM produces this directly from zero-padded weight
-// rows), so each 64-half chunk of a tile is exactly one TMA SWIZZLE_128B box.  O is written unpadded
-// ([b, s, h*d]) because it feeds the out-projection GEMM as a plain K-major A operand.
+// Layout: Q/K/V rows are tokens; every head owns d_pad (multiple of 16) consecutive halfs, the first d of which are
+// data and the rest zero (the projection GEMM produces this directly from zero-padded weight rows).  Shared-memory tiles
+// are whole 64-column chunks, each one TMA SWIZZLE_128B box; a box that runs past its head reads the next head's first
+// columns (never used: Q.K^T stops at d16, and P.V columns >= d are not stored) or, for the last head, the tensor map's
+// zero fill.  O is written unpadded ([b, s, h*d]) because it feeds the out-projection GEMM as a plain K-major A operand.
 //
-// One CTA = one 128-row Q tile of one (batch, head), kv consumed in tiles of 64.  320 threads:
-//   warp 0    TMA producer (Q once; K ring of 3, V ring of 2 — or K/V resident and Q tiles streaming, see `resident`)
-//   warp 1    TMEM allocator + single-thread tcgen05.mma issuer:  S[j%2] = Q K_j^T (M128 x N<=64 x K=d),
-//             O_h (+)= P_h V_h for the two 32-row halves h of the kv tile (M128 x N=d_pad x K=32 each; A = P straight from
-//             TMEM, where the softmax warps write it over their own S columns; V consumed MN-major from its TMA tile)
-//   warps 2-9 softmax.  Thread pair == query row: TMEM lane = (warp%4)*32 + lane; the two warps of a lane quarter
-//             take the two 32-column halves of the kv tile.
-// The two halves of a row are INDEPENDENT online-softmax streams: each has its own running maximum and its own
-// accumulator (O_a for kv rows 0-31 of every tile, O_b for rows 32-63), merged once at the end
-//   O = (O_a 2^(m_a-m) + O_b 2^(m_b-m)) / (l_a 2^(m_a-m) + l_b 2^(m_b-m)),   m = max(m_a, m_b).
-// That removes the per-tile cross-warp vote of a shared maximum (a 64-thread named barrier per tile cost 6 % of the
-// exp rate in isolation, tools/xu_probe.cu); the only per-tile agreement left is a warp-local __any_sync.
-// Softmax is single pass ("lazy max"): P = exp2(S*scale - m_used) uses the running maximum of earlier tiles; the
-// maximum of the produced P values is tracked on the packed 16-bit pairs (3-input VHMNMX), and only if it exceeds 2^8
-// for some lane of the warp (P would leave fp16's comfortable range) is the tile redone with an exact new maximum
-// after rescaling the warp's rows of O_h in TMEM — rare after the first tile.  S*scale - m is a packed FFMA2, each S
-// element is read from TMEM once (one 32-column load per thread and tile), and with a ones column in V (v_ones_col)
-// the row sums l_a, l_b come out of the P.V MMAs instead of CUDA-core adds.
-//
-// TMEM: S0 @ +0, S1 @ +64 (64 fp32 columns each), O_a @ +128, O_b @ +128 + d_pad.  P of tile t replaces S of tile t in
-// place: the warp of (lane quarter, half h) packs its 32 P values into the first 16 of its own 32 S columns (P_a @ +0,
-// P_b @ +32 of the buffer), so nobody overwrites what another warp still has to read, and P.V(t) is issued BEFORE
-// Q.K(t+2) refills the buffer (one thread's MMAs execute in order).  d_pad == 64: 256 columns and ~57 KB shared memory
-// (Q + K ring + V ring), two CTAs per SM.  (B200SD_ATTN_PTMEM=0 keeps the earlier form: P as fp16 in swizzled shared
-// memory, three buffers, Q.K issued first.)
-//
-// mbarrier phase discipline (parity waits alias if a waiter can fall two phases behind):
-//   o_full[pb] P.V of tile j commits to o_full[j%pb].  Waited by the softmax warps before a rescale of O and at the end, and
-//              (ring mode) by the producer for slot reuse; a commit fires when ALL MMAs its thread issued before it have
-//              completed, so it also covers the Q.K products issued earlier.  In the shared-memory-P form the order
-//              Q.K(j), P.V(j-2), Q.K(j+1), ... makes "S[j] ready" prove that P.V of tiles <= j-3 is complete: P[j%3] is
-//              free without a wait of its own (hence three P buffers there).
-//   p_full[pb] 8 warp arrivals; in ring mode + 1 arrival of the producer, whose expect_tx puts the bytes of K_{t+2} and V_t
-//              on the phase of tile t (see the producer): the MMA thread's one wait per tile covers P and its operands.
-//              Waiters: the MMA thread and (ring mode) the producer, neither of which can be lapped — a later phase needs
-//              S of a tile the MMA thread issues after this wait, and the producer's own arrival.
-//   s_full[2] / q_full / q_empty / o_free and resident mode's k_full / v_full: one waiting side, alternating with the
-//              signalling side.
-// All waits carry a suspend hint: a polling loop without it steals issue slots from the warps doing the exponentials
-// (measured: a polling TMA producer cost 25 % of this kernel's time).
+// One CTA = one 128-row Q tile of one (batch, head); 256 threads = two warpgroups, warpgroup w owns Q rows
+// [64w, 64w+64).  K / V are consumed in tiles of 64 rows through a ring of `stages` shared-memory slots that thread 0
+// refills by TMA (a slot is refilled once both warpgroups have released it).  Per kv tile and warpgroup:
+//   S = Q K^T        wgmma m64n64k16, A = Q and B = K both K-major in shared memory, S in registers
+//   online softmax   exact running maximum per row (the four threads of a row agree through two shuffles), P = 2^(S*scale*log2 e - m)
+//   O += P V         wgmma m64n(64*chunks)k16 with A = P from registers (the S accumulator fragment is the A fragment)
+//                    and B = V MN-major in shared memory
+// The row sums are accumulated in fp32 registers, so the ones column a caller may place in V (v_ones_col) is not needed
+// and its output column is not stored.
 #include <cstddef>
 #include <cstdlib>
 
 #include "tc_common.cuh"
+#include "wgmma.cuh"
 #include "b200sd_internal.h"
 #include "pdl.cuh"
 
 namespace b200sd {
 
-constexpr int kSoftmaxWarps = 8;
-constexpr int kSoftmaxThreads = 32 * kSoftmaxWarps;
-constexpr int kAttnThreads = 64 + kSoftmaxThreads;
+constexpr int kAttnThreads = 256;                    // two warpgroups
 constexpr int kQTile = 128;
 constexpr int kKv = 64;                              // kv rows per tile
-constexpr int kSBufs = 2;                            // S buffers in TMEM
+constexpr int kMaxStages = 3;
 constexpr uint32_t kQChunkBytes = kQTile * 128;      // 128 rows x 64 halfs
 constexpr uint32_t kKvChunkBytes = kKv * 128;        // 64 rows x 64 halfs
-constexpr uint32_t kPBytes = kQTile * kKv * 2;       // one K-major SWIZZLE_128B atom: 128 rows x 64 halfs
-constexpr int kMaxRing = 4;
-constexpr int kMaxPBufs = 3;
 
 struct AttnParams {
   int B, heads, Sq, Skv, d, d_pad;
-  int d16;           // d rounded up to 16 (MMA K of Q.K^T; O columns that carry data)
-  int dpv;           // MMA N of P.V = d_pad (whole 64-wide MN-major swizzle atoms; pad columns of V are zero)
-  int chunks;        // d_pad / 64
-  int p_bufs;        // P buffers in shared memory (2 or 3)
-  int k_stages, v_stages;  // K / V ring depths (<= kMaxRing)
-  int tmem_cols;
-  int l_col;         // >= 0: V carries a ones column at l_col (== d) and O_h[:, l_col] is the softmax denominator
-  int resc_cols;     // O columns touched by a rescale (multiple of 16, covers l_col)
+  int d16;           // d rounded up to 16 (MMA K of Q.K^T)
+  int chunks;        // 64-column chunks per head tile
+  int stages;        // K / V ring slots
   float scale_log2;  // softmax scale * log2(e)
   void* O;
   long long ldo;
-  int is_bf16;
-  long long* trace;  // debug: clock64 timeline of one CTA ([16 events][nkv]), or null
-  int resident;      // 1: K / V fit in shared memory (Skv <= 128): loaded once, the CTA walks `qpc` Q tiles
-  int qpc;           // Q tiles per CTA (1 in ring mode)
-  int q_bufs;        // Q buffers in shared memory (2 in resident mode: the next Q tile is prefetched)
-  int num_q_tiles;
-  int p_tmem;        // P is written back over its own S columns in TMEM (no shared-memory P, no proxy fence)
-  int p_smem;        // P buffers that exist in shared memory: p_bufs, or 0 with p_tmem
 };
 
-struct __align__(16) AttnShared {
-  uint64_t q_full[2], q_empty[2];
-  uint64_t o_free;  // resident mode: the epilogue of a Q tile has read both accumulators
-  uint64_t k_full[kMaxRing], v_full[kMaxRing];  // resident mode only (ring mode: the loads land on p_full)
-  uint64_t s_full[kSBufs], p_full[kMaxPBufs], o_full[kMaxPBufs];
-  uint32_t tmem_base;
-  uint32_t pad;
-  float xm[2][kQTile];  // final merge: running maxima / row sums of the two column halves
-  float xl[2][kQTile];
+struct __align__(8) AttnShared {
+  uint64_t q_full;
+  uint64_t kv_full[kMaxStages];
+  uint64_t kv_empty[kMaxStages];  // one arrival per warpgroup
 };
 
 template <bool kBf16>
@@ -116,747 +64,180 @@ __device__ __forceinline__ uint32_t pack_h2(float a, float b) {
   }
 }
 
-__device__ __forceinline__ float fmax3(float a, float b, float c) {
-  float d;
-  asm("max.f32 %0, %1, %2, %3;" : "=f"(d) : "f"(a), "f"(b), "f"(c));
-  return d;
-}
-
-__device__ __forceinline__ void sts128(uint32_t addr, uint32_t a, uint32_t b, uint32_t c, uint32_t d) {
-  asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(addr), "r"(a), "r"(b), "r"(c), "r"(d) : "memory");
-}
-
-// named barriers 1..4: the two warps (64 threads) that share one TMEM lane quarter, i.e. the thread pairs of 32 rows
-__device__ __forceinline__ void pair_bar_sync(int quarter) {
-  asm volatile("bar.sync %0, 64;" ::"r"(quarter + 1) : "memory");
-}
-
-// maximum of my 32 columns [col0, col0+32) of the S tile (raw logits); kv columns >= nvalid ignored
-template <bool kFull>
-__device__ __forceinline__ float half_row_max(uint32_t tmem_row, int col0, int nvalid) {
-  float mx = -INFINITY;
-#pragma unroll
-  for (int s = 0; s < 2; ++s) {
-    const int cbase = col0 + s * 16;
-    uint32_t v[16];
-    tmem_ld_x16(tmem_row + cbase, v);  // warp-collective: never skipped, masked instead
-    tmem_ld_wait();
-#pragma unroll
-    for (int i = 0; i < 16; i += 2) {
-      float a = __uint_as_float(v[i]), b2 = __uint_as_float(v[i + 1]);
-      if (!kFull) {
-        if (cbase + i >= nvalid) a = -INFINITY;
-        if (cbase + i + 1 >= nvalid) b2 = -INFINITY;
-      }
-      mx = fmax3(mx, a, b2);
-    }
-  }
-  return mx;
-}
-
-// Blackwell packed fp32 FMA (FFMA2): (a.x, a.y) * (b.x, b.y) + (c.x, c.y)
-__device__ __forceinline__ uint64_t pack_f2(uint32_t lo, uint32_t hi) {
-  uint64_t r;
-  asm("mov.b64 %0, {%1, %2};" : "=l"(r) : "r"(lo), "r"(hi));
-  return r;
-}
-__device__ __forceinline__ void ffma2(float& x, float& y, uint32_t a_lo, uint32_t a_hi, uint64_t b, uint64_t c) {
-  uint64_t d;
-  asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(d) : "l"(pack_f2(a_lo, a_hi)), "l"(b), "l"(c));
-  uint32_t lo, hi;
-  asm("mov.b64 {%0, %1}, %2;" : "=r"(lo), "=r"(hi) : "l"(d));
-  x = __uint_as_float(lo);
-  y = __uint_as_float(hi);
-}
-// running maximum over packed 16-bit pairs (two of these fuse into one 3-input VHMNMX)
-template <bool kBf16>
-__device__ __forceinline__ uint32_t max3_h2(uint32_t m, uint32_t a, uint32_t b) {
-  uint32_t r;
-  if constexpr (kBf16) {
-    asm("max.bf16x2 %0, %1, %2;" : "=r"(r) : "r"(m), "r"(a));
-    asm("max.bf16x2 %0, %1, %2;" : "=r"(r) : "r"(r), "r"(b));
-  } else {
-    asm("max.f16x2 %0, %1, %2;" : "=r"(r) : "r"(m), "r"(a));
-    asm("max.f16x2 %0, %1, %2;" : "=r"(r) : "r"(r), "r"(b));
-  }
-  return r;
-}
-template <bool kBf16>
-__device__ __forceinline__ float h2_hmax(uint32_t v) {
-  if constexpr (kBf16) {
-    __nv_bfloat162 h = *reinterpret_cast<__nv_bfloat162*>(&v);
-    return fmaxf(__low2float(h), __high2float(h));
-  } else {
-    __half2 h = *reinterpret_cast<__half2*>(&v);
-    return fmaxf(__low2float(h), __high2float(h));
-  }
-}
-
-// exp2 on the FMA pipe for a share of the elements (the MUFU unit, 16 ex2 / clock / SM, is the softmax warps' busiest
-// pipe): x = n + f with n = round(x), f in [-0.5, 0.5]; 2^f by a degree-3 minimax polynomial (relative error 7.5e-5, a
-// third of the rounding error of the fp16 P value it becomes), 2^n by adding n to the exponent field.  Packed fp32 (FFMA2)
-// for the pair; every B200SD_ATTN_POLY_STRIDE-th pair of a thread's 16 takes this path (0: none).
-// Measured at the batch-16 self-attention shape: stride 0 0.773 ms, 4 (25 %) 0.766 ms, 3 0.770 ms, 2 (50 %) 0.839 ms — the
-// 13 FMA-pipe instructions per pair cost the issue slots the 2 MUFU instructions free, so it stays off.
-#ifndef B200SD_ATTN_POLY_STRIDE
-#define B200SD_ATTN_POLY_STRIDE 0
-#endif
-__device__ __forceinline__ uint64_t ffma2_raw(uint64_t a, uint64_t b, uint64_t c) {
-  uint64_t d;
-  asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(d) : "l"(a), "l"(b), "l"(c));
-  return d;
-}
-__device__ __forceinline__ uint64_t splat_f2(float v) { return pack_f2(__float_as_uint(v), __float_as_uint(v)); }
-__device__ __forceinline__ void exp2_poly2(float& ea, float& eb, float xa, float xb) {
-  xa = fminf(fmaxf(xa, -125.f), 126.f);
-  xb = fminf(fmaxf(xb, -125.f), 126.f);
-  const uint64_t x2 = pack_f2(__float_as_uint(xa), __float_as_uint(xb));
-  const uint64_t one2 = splat_f2(1.0f), magic2 = splat_f2(12582912.0f), nmagic2 = splat_f2(-12582912.0f);
-  const uint64_t r2 = ffma2_raw(x2, one2, magic2);         // low mantissa bits = round(x)
-  const uint64_t n2 = ffma2_raw(r2, one2, nmagic2);        // round(x) as a float (exact)
-  const uint64_t f2 = ffma2_raw(n2, splat_f2(-1.0f), x2);  // x - round(x)
-  uint64_t p2 = ffma2_raw(splat_f2(0.05517164245247841f), f2, splat_f2(0.2426111251115799f));
-  p2 = ffma2_raw(p2, f2, splat_f2(0.6932609677314758f));
-  p2 = ffma2_raw(p2, f2, splat_f2(0.9999280571937561f));
-  uint32_t pa, pb, ra, rb;
-  asm("mov.b64 {%0, %1}, %2;" : "=r"(pa), "=r"(pb) : "l"(p2));
-  asm("mov.b64 {%0, %1}, %2;" : "=r"(ra), "=r"(rb) : "l"(r2));
-  ea = __uint_as_float(pa + (ra << 23));
-  eb = __uint_as_float(pb + (rb << 23));
-}
-
-// exp2 of a pair on the half-precision FMA pipe, straight to the packed fp16 P value (no MUFU, no separate pack):
-//   x -> half2, clamped to >= -13;  r = x + 1551 (fp16 ulp is 1 there: the low mantissa bits of r are round(x) + 527);
-//   n = r - 1551, f = x - n in [-0.5, 0.5];  2^f by a degree-3 polynomial (3 HFMA2);  2^n by adding n to the exponent field:
-//   bits = p + ((r & 0x3f) << 10) - (15 << 10) per 16-bit lane ((527 + n) & 0x3f == n + 15; no lane carries: p < 0x3dff).
-// The MUFU unit (16 ex2 / clock / SM) is this kernel's busiest pipe at 66-69 %; B200SD_ATTN_H2POLY_MASK says which of a
-// thread's 16 pairs per tile take this path instead (bit i = pair i; 0 = none).  fp16 only: bf16's 7 mantissa bits cannot
-// carry x.  Accuracy (numpy emulation): rms relative error 2.7e-4 for x in [-2, 0] (MUFU + pack: 2.1e-4), up to 0.3 % where
-// |x| > 8 (x itself is rounded to half there).
-// Measured (round 2, batch-64 self-attention shape, S = 4096, d = 40; tools/gpu_attn_exp.sh): none 2.811 ms; 2 of 16 pairs
-// 2.549; 3 of 16 2.503; 4 of 16 2.453 (pairs 3, 7, 11, 15) .. 2.501 (pairs 0, 4, 8, 12); 6 of 16 2.583; 8 of 16 2.623;
-// 12 of 16 2.866 — the first few offloaded pairs relieve the MUFU queue (ncu: mio_throttle was the second largest stall),
-// beyond a quarter the extra issue slots cost more.  Parity with 4 of 16: one SD1.5 UNet evaluation rel-rms 1.45e-3 (1.44e-3
-// without), images of whole sampler runs unchanged (max 1 LSB, mean 0.09-0.12, 88-91 % identical).
-#ifndef B200SD_ATTN_H2POLY_MASK
-#define B200SD_ATTN_H2POLY_MASK 0x8888
-#endif
-__device__ __forceinline__ uint32_t exp2_h2_poly(float xa, float xb) {
-  uint32_t x, r, n, f, p;
-  asm("cvt.rn.f16x2.f32 %0, %1, %2;" : "=r"(x) : "f"(xb), "f"(xa));           // low half = xa
-  asm("max.f16x2 %0, %1, %2;" : "=r"(x) : "r"(x), "r"(0xCA80CA80u));            // >= -13
-  asm("add.rn.f16x2 %0, %1, %2;" : "=r"(r) : "r"(x), "r"(0x660F660Fu));         // + 1551
-  asm("add.rn.f16x2 %0, %1, %2;" : "=r"(n) : "r"(r), "r"(0xE60FE60Fu));         // - 1551 = round(x)
-  asm("sub.rn.f16x2 %0, %1, %2;" : "=r"(f) : "r"(x), "r"(n));
-  asm("fma.rn.f16x2 %0, %1, %2, %3;" : "=r"(p) : "r"(0x2B102B10u), "r"(f), "r"(0x33C333C3u));
-  asm("fma.rn.f16x2 %0, %1, %2, %3;" : "=r"(p) : "r"(p), "r"(f), "r"(0x398C398Cu));
-  asm("fma.rn.f16x2 %0, %1, %2, %3;" : "=r"(p) : "r"(p), "r"(f), "r"(0x3C003C00u));
-  return p + ((r & 0x003F003Fu) << 10) - 0x3C003C00u;
-}
-
-// P values above this mean the tile's maximum exceeds the running maximum by more than 2^8: redo with a new maximum
-constexpr float kPRedo = 256.0f;
-
-
-
-// debug timeline (b200sd_debug_attention_trace; build with -DB200SD_ATTN_TRACE_ENABLE=1): CTA (3, 2, 1) stamps per-tile
-// events of softmax warp 2 and the MMA thread.  Compiled out by default: the trace pointer costs two registers in a
-// kernel that sits exactly at its register cap.
-#ifndef B200SD_ATTN_TRACE_ENABLE
-#define B200SD_ATTN_TRACE_ENABLE 0
-#endif
-#if B200SD_ATTN_TRACE_ENABLE
-#define ATTN_TRACE(ev, j) \
-  do { if (trace) trace[(ev) * 64 + ((j) & 63)] = clock64(); } while (0)
-#define ATTN_TRACE_PTR(cond) long long* trace = (cond) ? p.trace : nullptr
-#else
-#define ATTN_TRACE(ev, j) do { } while (0)
-#define ATTN_TRACE_PTR(cond) do { } while (0)
-#endif
-
-// my 32 columns of one S tile -> P values packed into pk[16]; returns true when some P value left the comfortable range
-template <bool kFull, bool kBf16, bool kSum>
-__device__ __forceinline__ bool softmax32(const uint32_t (&v)[32], uint32_t (&pk)[16], int col0, int nvalid,
-                                          float scale_log2, float m_used, float& lsum) {
-  const uint64_t scale2 = pack_f2(__float_as_uint(scale_log2), __float_as_uint(scale_log2));
-  const uint64_t negm2 = pack_f2(__float_as_uint(-m_used), __float_as_uint(-m_used));
-  float acc = 0.f;
-#pragma unroll
-  for (int i = 0; i < 32; i += 2) {
-    float xa, xb;
-    ffma2(xa, xb, v[i], v[i + 1], scale2, negm2);
-    if constexpr (!kBf16 && !kSum && B200SD_ATTN_H2POLY_MASK != 0) {
-      if ((B200SD_ATTN_H2POLY_MASK >> (i >> 1)) & 1) {   // compile-time after unrolling
-        uint32_t e2 = exp2_h2_poly(xa, xb);
-        if (!kFull) {
-          if (col0 + i >= nvalid) e2 &= 0xFFFF0000u;
-          if (col0 + i + 1 >= nvalid) e2 &= 0x0000FFFFu;
-        }
-        pk[i >> 1] = e2;
-        continue;
-      }
-    }
-    float ea, eb;
-    if (B200SD_ATTN_POLY_STRIDE > 0 && ((i >> 1) % (B200SD_ATTN_POLY_STRIDE > 0 ? B200SD_ATTN_POLY_STRIDE : 1)) ==
-                                           (B200SD_ATTN_POLY_STRIDE > 0 ? B200SD_ATTN_POLY_STRIDE : 1) - 1) {
-      exp2_poly2(ea, eb, xa, xb);
-    } else {
-      ea = fast_exp2(xa);
-      eb = fast_exp2(xb);
-    }
-    if (!kFull) {
-      if (col0 + i >= nvalid) ea = 0.f;
-      if (col0 + i + 1 >= nvalid) eb = 0.f;
-    }
-    if constexpr (kSum) acc += ea + eb;
-    pk[i >> 1] = pack_h2<kBf16>(ea, eb);
-  }
-  uint32_t pm0 = 0u, pm1 = 0u;  // two chains
-#pragma unroll
-  for (int i = 0; i < 16; i += 4) {
-    pm0 = max3_h2<kBf16>(pm0, pk[i], pk[i + 1]);
-    pm1 = max3_h2<kBf16>(pm1, pk[i + 2], pk[i + 3]);
-  }
-  if constexpr (kSum) lsum += acc;
-  return fmaxf(h2_hmax<kBf16>(pm0), h2_hmax<kBf16>(pm1)) > kPRedo;
-}
-// four 16-byte chunks of my row of the swizzled P atom; p_row = shared-space address of the row, rx = row & 7
-__device__ __forceinline__ void p_store32(const uint32_t (&pk)[16], uint32_t p_row, uint32_t rx, int col0) {
-  const uint32_t chunk0 = static_cast<uint32_t>(col0 >> 3);  // 8 halfs per 16-byte chunk
-#pragma unroll
-  for (int c = 0; c < 4; ++c)
-    sts128(p_row + (((chunk0 + c) ^ rx) << 4), pk[4 * c], pk[4 * c + 1], pk[4 * c + 2], pk[4 * c + 3]);
-}
-
-template <bool kBf16, bool kSum>
-__device__ __forceinline__ void softmax_warps(const AttnParams& p, AttnShared* sh, uint8_t* sP, uint32_t tmem_base,
-                                              int warp, int lane, int first_qt, int n_items, int head, int b, int nkv) {
-  const int quarter = warp & 3;
-  const int half = (warp - 2) >> 2;   // which 32-column half of the kv tile (and which accumulator) is mine
-  const int r = quarter * 32 + lane;  // query row in the tile == TMEM lane
-  const uint32_t lane_base = static_cast<uint32_t>(quarter * 32) << 16;
-  const uint32_t oa_row = tmem_base + static_cast<uint32_t>(kSBufs * kKv) + lane_base;
-  const uint32_t ob_row = oa_row + static_cast<uint32_t>(p.dpv);
-  const uint32_t o_row = half == 0 ? oa_row : ob_row;  // the accumulator my P values feed
-  const uint32_t p_row0 = smem_u32(sP) + static_cast<uint32_t>(r) * 128u;
-  const uint32_t rx = static_cast<uint32_t>(r) & 7u;
-  const uint32_t a_s_full = smem_u32(&sh->s_full[0]);
-  const uint32_t a_p_full = smem_u32(&sh->p_full[0]);
-  const uint32_t a_o_full = smem_u32(&sh->o_full[0]);
-  const uint32_t a_o_free = smem_u32(&sh->o_free);
-  const int col0 = half * 32;
-  const int p_bufs = p.p_bufs, skv = p.Skv;
-  const float scale_log2 = p.scale_log2;
-  const bool has_b = skv > 32;  // kv rows 32-63 never exist when Skv <= 32: O_b is never written
-  ATTN_TRACE_PTR(p.trace && blockIdx.x == 3 && blockIdx.y == 2 && blockIdx.z == 1 && warp == 2 && lane == 0);
-  // The kv tiles of all the CTA's Q tiles ("items") form ONE stream t = 0, 1, ...: S / P buffers and barrier phases
-  // simply continue across items.
-  int t = 0;
-  int pb = 0;                // P buffer of tile t and the parity of its current barrier phase
-  uint32_t p_par = 0;
-  for (int it = 0; it < n_items; ++it) {
-    const int q0 = (first_qt + it) * kQTile;
-    float m_used = -INFINITY;  // scaled log2 domain; running maximum of MY half of the row
-    float l = 0.f;
-    for (int j = 0; j < nkv; ++j, ++t) {
-      const int sb = t & 1;
-      const int nvalid = min(kKv, skv - j * kKv);
-      const bool full = nvalid == kKv;
-      const uint32_t s_row = tmem_base + static_cast<uint32_t>(sb * kKv) + lane_base;
-      const uint32_t p_row = p_row0 + static_cast<uint32_t>(pb) * kPBytes;
-      ATTN_TRACE(0, t);
-      mbar_wait_a(a_s_full + sb * 8, (static_cast<uint32_t>(t) >> 1) & 1u, 17);
-      tc_fence_after();
-      ATTN_TRACE(1, t);
-      if (j == 0) m_used = (full ? half_row_max<true>(s_row, col0, nvalid) : half_row_max<false>(s_row, col0, nvalid)) * scale_log2;
-      uint32_t v[32], pk[16];
-      tmem_ld_x32(s_row + col0, v);
-      tmem_ld_wait();
-      ATTN_TRACE(2, t);
-      float lsum = 0.f;
-      const bool over = full ? softmax32<true, kBf16, kSum>(v, pk, col0, nvalid, scale_log2, m_used, lsum)
-                             : softmax32<false, kBf16, kSum>(v, pk, col0, nvalid, scale_log2, m_used, lsum);
-      // P[pb] was last read by P.V of tile t - p_bufs, complete because S[t] is (see the header)
-      ATTN_TRACE(3, t);
-      if (__any_sync(0xffffffffu, over)) {
-        // rare path (warp-uniform, the TMEM accesses are warp-collective): some row of this warp saw its maximum move
-        // by more than 2^8.  Lanes that did not overflow run it with alpha ~ 1.
-        const float mx = (full ? half_row_max<true>(s_row, col0, nvalid) : half_row_max<false>(s_row, col0, nvalid)) * scale_log2;
-        const float m_new = fmaxf(m_used, mx);
-        const float alpha = fast_exp2(m_used - m_new);
-        if (j > 0) {
-          // P.V of the previous tile must have landed in O_h
-          mbar_wait_a(a_o_full + (pb == 0 ? p_bufs - 1 : pb - 1) * 8, pb == 0 ? p_par ^ 1u : p_par, 18);
-          tc_fence_after();
-          for (int c = 0; c < p.resc_cols / 16; ++c) {
-            uint32_t o[16];
-            tmem_ld_x16(o_row + c * 16, o);
-            tmem_ld_wait();
-#pragma unroll
-            for (int i = 0; i < 16; ++i) o[i] = __float_as_uint(__uint_as_float(o[i]) * alpha);
-            tmem_st_x16(o_row + c * 16, o);
-          }
-          tmem_st_wait();
-        }
-        l *= alpha;
-        m_used = m_new;
-        lsum = 0.f;
-        tmem_ld_x32(s_row + col0, v);
-        tmem_ld_wait();
-        if (full) softmax32<true, kBf16, kSum>(v, pk, col0, nvalid, scale_log2, m_used, lsum);
-        else      softmax32<false, kBf16, kSum>(v, pk, col0, nvalid, scale_log2, m_used, lsum);
-      }
-      if (p.p_tmem) {
-        // my 32 P values, packed in pairs, over the first 16 of my own 32 S columns: TMEM lane = query row, column j of
-        // the half = kv rows 2j, 2j+1 — exactly the A-operand layout of the P.V MMA.  Q.K of tile t+2 overwrites the buffer
-        // only after P.V of this tile (same issuing thread, in order).
-        tmem_st_x16(s_row + col0, pk);
-        tmem_st_wait();
-      } else {
-        p_store32(pk, p_row, rx, col0);
-      }
-      l += lsum;
-      ATTN_TRACE(5, t);
-      if (!p.p_tmem) fence_proxy_async_smem();
-      tc_fence_before();
-      __syncwarp();
-      ATTN_TRACE(6, t);
-      if (lane == 0) mbar_arrive_a(a_p_full + pb * 8);  // one arrival per warp
-      if (++pb == p_bufs) {
-        pb = 0;
-        p_par ^= 1u;
-      }
-    }
-    // ---- epilogue of this Q tile: merge the two halves of every row, O / l -> global (the pair splits the chunks) ----
-    mbar_wait_a(a_o_full + (pb == 0 ? p_bufs - 1 : pb - 1) * 8, pb == 0 ? p_par ^ 1u : p_par, 19);  // P.V of tile t-1
-    tc_fence_after();
-    if constexpr (!kSum) {
-      uint32_t o[16];
-      tmem_ld_x16(o_row + (p.l_col / 16) * 16, o);
-      tmem_ld_wait();
-      l = 0.f;
-#pragma unroll
-      for (int i = 0; i < 16; ++i)
-        if (i == (p.l_col & 15)) l = __uint_as_float(o[i]);
-    }
-    if (half == 1 && !has_b) {
-      l = 0.f;
-      m_used = -INFINITY;
-    }
-    if (it > 0) pair_bar_sync(quarter);  // my partner has read the previous Q tile's exchange values
-    sh->xm[half][r] = m_used;
-    sh->xl[half][r] = l;
-    pair_bar_sync(quarter);
-    const float m_o = sh->xm[half ^ 1][r], l_o = sh->xl[half ^ 1][r];
-    const float m = fmaxf(m_used, m_o);
-    const float a_me = fast_exp2(m_used - m), a_ot = fast_exp2(m_o - m);  // 2^(-inf) = 0 for an empty half
-    const float inv_l = 1.0f / (l * a_me + l_o * a_ot);
-    const float wa = (half == 0 ? a_me : a_ot) * inv_l, wb = (half == 0 ? a_ot : a_me) * inv_l;
-    const int srow = q0 + r;
-    const bool valid = srow < p.Sq;
-    uint8_t* orow = reinterpret_cast<uint8_t*>(p.O) +
-                    ((static_cast<long long>(b) * p.Sq + (valid ? srow : 0)) * p.ldo + static_cast<long long>(head) * p.d) * 2;
-    for (int c = half; c < p.d16 / 16; c += 2) {
-      uint32_t oa[16], ob[16];
-      tmem_ld_x16(oa_row + c * 16, oa);
-      tmem_ld_x16(ob_row + c * 16, ob);
-      tmem_ld_wait();
-      uint32_t h[8];
-#pragma unroll
-      for (int i = 0; i < 8; ++i) {
-        float x0 = __uint_as_float(oa[2 * i]) * wa, x1 = __uint_as_float(oa[2 * i + 1]) * wa;
-        if (has_b) {
-          x0 = fmaf(__uint_as_float(ob[2 * i]), wb, x0);
-          x1 = fmaf(__uint_as_float(ob[2 * i + 1]), wb, x1);
-        }
-        h[i] = pack_h2<kBf16>(x0, x1);
-      }
-      if (valid) {
-        if (c * 16 + 8 <= p.d) *reinterpret_cast<uint4*>(orow + c * 32) = make_uint4(h[0], h[1], h[2], h[3]);
-        if (c * 16 + 16 <= p.d) *reinterpret_cast<uint4*>(orow + c * 32 + 16) = make_uint4(h[4], h[5], h[6], h[7]);
-      }
-    }
-    // the accumulators may be overwritten by the next Q tile's first P.V
-    tc_fence_before();
-    __syncwarp();
-    if (lane == 0) mbar_arrive_a(a_o_free);
-  }
-}
-
-__global__ void __launch_bounds__(kAttnThreads, 2)
+template <int kChunks, bool kBf16>
+__global__ void __launch_bounds__(kAttnThreads, 1)
 attention_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
                     const __grid_constant__ CUtensorMap tmV, const AttnParams p) {
+  constexpr int kDv = 64 * kChunks;  // MMA N of P.V
+  constexpr uint32_t kKvBytes = kChunks * kKvChunkBytes;
   extern __shared__ uint8_t smem_raw[];
   pdl_trigger();  // pdl.cuh: the next kernel's prologue may overlap this kernel's tail
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  const uint32_t q_bytes = static_cast<uint32_t>(p.chunks) * kQChunkBytes;
-  const uint32_t kv_bytes = static_cast<uint32_t>(p.chunks) * kKvChunkBytes;
-  uint8_t* sQ = smem;                                   // q_bufs x (128 rows x d_pad)
-  uint8_t* sP = sQ + static_cast<size_t>(p.q_bufs) * q_bytes;  // p_bufs x 16 KB
-  uint8_t* sK = sP + p.p_smem * kPBytes;
-  uint8_t* sV = sK + p.k_stages * kv_bytes;
-  AttnShared* sh = reinterpret_cast<AttnShared*>(sV + p.v_stages * kv_bytes);
+  uint8_t* sQ = smem;                                   // chunks x (128 rows x 64)
+  uint8_t* sK = sQ + kChunks * kQChunkBytes;            // stages x chunks x (64 rows x 64)
+  uint8_t* sV = sK + p.stages * kKvBytes;
+  AttnShared* sh = reinterpret_cast<AttnShared*>(sV + p.stages * kKvBytes);
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
-  const int first_qt = blockIdx.x * p.qpc;               // this CTA's Q tiles: first_qt .. first_qt + n_items - 1
-  const int n_items = min(p.qpc, p.num_q_tiles - first_qt);
+  const int wg = warp >> 2;
+  const int qt = blockIdx.x;
   const int head = blockIdx.y;
   const int b = blockIdx.z;
   const int nkv = (p.Skv + kKv - 1) / kKv;
   const int col0 = head * p.d_pad;
-  const bool resident = p.resident != 0;                  // K / V of this (batch, head) stay in shared memory
+  const bool loader = threadIdx.x == 0;
 
-  if (warp == 0 && lane == 0) {
+  if (loader) {
     tma_prefetch_desc(&tmQ);
     tma_prefetch_desc(&tmK);
     tma_prefetch_desc(&tmV);
-    for (int s = 0; s < 2; ++s) {
-      mbar_init(&sh->q_full[s], 1);
-      mbar_init(&sh->q_empty[s], 1);
+    mbar_init(&sh->q_full, 1);
+    for (int s = 0; s < kMaxStages; ++s) {
+      mbar_init(&sh->kv_full[s], 1);
+      mbar_init(&sh->kv_empty[s], 2);
     }
-    for (int s = 0; s < kMaxRing; ++s) {
-      mbar_init(&sh->k_full[s], 1);
-      mbar_init(&sh->v_full[s], 1);
-    }
-    for (int s = 0; s < kSBufs; ++s) mbar_init(&sh->s_full[s], 1);
-    for (int s = 0; s < kMaxPBufs; ++s) {
-      mbar_init(&sh->p_full[s], resident ? kSoftmaxWarps : kSoftmaxWarps + 1);  // ring mode: + the producer's expect_tx
-      mbar_init(&sh->o_full[s], 1);
-    }
-    mbar_init(&sh->o_free, kSoftmaxWarps);
     fence_mbar_init();
   }
-  if (warp == 1) tmem_alloc(&sh->tmem_base, static_cast<uint32_t>(p.tmem_cols));
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = sh->tmem_base;  // S0 @ +0, S1 @ +64, O_a @ +128, O_b @ +128 + dpv
   pdl_wait();  // Q / K / V come from the preceding projection GEMM
 
-  if (warp == 0) {
-    // ------------------------------------ TMA producer ------------------------------------
-    // The warp stays converged (all lanes wait) and one elected lane issues, so the TMA instructions take warp-uniform
-    // operands without a per-instruction broadcast loop.
-    const bool leader = elect_one();
-    const uint32_t bar0 = warp_uniform(smem_u32(sh));
-    const uint32_t a_q_empty = bar0 + static_cast<uint32_t>(offsetof(AttnShared, q_empty));
-    const int k_stages = p.k_stages, v_stages = p.v_stages, chunks = p.chunks;
-    if (resident) {
-      // K / V (at most two tiles each) are loaded once; Q tiles stream through two buffers, one tile ahead
-      if (leader) {
-        for (int j = 0; j < nkv; ++j) {
-          mbar_arrive_expect_tx(&sh->k_full[j], kv_bytes);
-          for (int c = 0; c < chunks; ++c)
-            tma_load_3d(sK + j * kv_bytes + c * kKvChunkBytes, &tmK, &sh->k_full[j], col0 + c * 64, j * kKv, b);
-        }
-      }
-      for (int it = 0; it < n_items; ++it) {
-        const int qs = it & 1;
-        mbar_wait_a(a_q_empty + static_cast<uint32_t>(qs) * 8u, ((static_cast<uint32_t>(it) >> 1) & 1u) ^ 1u, 10);
-        if (leader) {
-          mbar_arrive_expect_tx(&sh->q_full[qs], q_bytes);
-          for (int c = 0; c < chunks; ++c)
-            tma_load_3d(sQ + qs * q_bytes + c * kQChunkBytes, &tmQ, &sh->q_full[qs], col0 + c * 64,
-                        (first_qt + it) * kQTile, b);
-          if (it == 0) {
-            for (int j = 0; j < nkv; ++j) {
-              mbar_arrive_expect_tx(&sh->v_full[j], kv_bytes);
-              for (int c = 0; c < chunks; ++c)
-                tma_load_3d(sV + j * kv_bytes + c * kKvChunkBytes, &tmV, &sh->v_full[j], col0 + c * 64, j * kKv, b);
-            }
-          }
-        }
-      }
-    } else {
-      // Ring mode (one Q tile per CTA).  Q, K_0 and K_1 land on q_full.  After that the operands the MMA thread needs once
-      // the softmax warps have delivered P_t — K_{t+2} for S[t+2] and V_t for P_t.V_t — are loaded as "pair t", and their
-      // bytes are expected on p_full of tile t itself: the barrier the MMA thread waits on anyway then also covers the
-      // loads, and the ring needs no full/empty barriers of its own (every mbarrier operation costs the issuing thread
-      // 150-350 clocks even when it does not block; the MMA thread's instruction stream is the kernel's critical path).
-      //   slots:  K_j in slot j % 3, V_j in slot j % 2.  Pair t overwrites K_{t-1} and V_{t-2}; Q.K of tile t-1 was issued
-      //           before P.V of tile t-3 and a commit covers every MMA its thread issued before it, so o_full(t-2) (or
-      //           o_full(0) for the K tiles used by the two start-up Q.K products) frees both.
-      //   phases: the producer arrives on p_full[t % pb] for tile t only after observing the phase of tile t-pb complete.
-      //           As an extra waiter on o_full / p_full it cannot be lapped: a later phase of either barrier needs
-      //           p_full of a tile this thread has not arrived for yet.
-      const uint32_t a_p_full = bar0 + static_cast<uint32_t>(offsetof(AttnShared, p_full));
-      const uint32_t a_o_full = bar0 + static_cast<uint32_t>(offsetof(AttnShared, o_full));
-      const int p_bufs = p.p_bufs;
-      const int pre = min(kSBufs, nkv);
-      if (leader) {
-        mbar_arrive_expect_tx(&sh->q_full[0], q_bytes + static_cast<uint32_t>(pre) * kv_bytes);
-        for (int c = 0; c < chunks; ++c)
-          tma_load_3d(sQ + c * kQChunkBytes, &tmQ, &sh->q_full[0], col0 + c * 64, first_qt * kQTile, b);
-        for (int j = 0; j < pre; ++j)
-          for (int c = 0; c < chunks; ++c)
-            tma_load_3d(sK + j * kv_bytes + c * kKvChunkBytes, &tmK, &sh->q_full[0], col0 + c * 64, j * kKv, b);
-      }
-      int pb = 0, k_st = pre % k_stages, v_st = 0;   // P buffer of tile t; ring slots of K_{t+2} and V_t
-      int ob = 0, lb = 0;                            // P buffers of tiles t-2 (o_full wait) and t-pb (p_full wait)
-      uint32_t o_par = 0, l_par = 0;
-      for (int t = 0; t < nkv; ++t) {
-        if (t >= 1) {  // slots free: P.V of tile max(t-2, 0) and everything issued before it has completed
-          mbar_wait_a(a_o_full + static_cast<uint32_t>(ob) * 8u, o_par, 11);
-          if (t >= 2 && ++ob == p_bufs) {
-            ob = 0;
-            o_par ^= 1u;
-          }
-        }
-        if (t >= p_bufs) {  // p_full[pb] has finished the phase of tile t - p_bufs: my arrival counts for tile t
-          mbar_wait_a(a_p_full + static_cast<uint32_t>(lb) * 8u, l_par, 12);
-          if (++lb == p_bufs) {
-            lb = 0;
-            l_par ^= 1u;
-          }
-        }
-        const bool has_k = t + kSBufs < nkv;
-        if (leader) {
-          mbar_arrive_expect_tx(&sh->p_full[pb], has_k ? 2u * kv_bytes : kv_bytes);
-          if (has_k)
-            for (int c = 0; c < chunks; ++c)
-              tma_load_3d(sK + k_st * kv_bytes + c * kKvChunkBytes, &tmK, &sh->p_full[pb], col0 + c * 64,
-                          (t + kSBufs) * kKv, b);
-          for (int c = 0; c < chunks; ++c)
-            tma_load_3d(sV + v_st * kv_bytes + c * kKvChunkBytes, &tmV, &sh->p_full[pb], col0 + c * 64, t * kKv, b);
-        }
-        if (++pb == p_bufs) pb = 0;
-        if (++k_st == k_stages) k_st = 0;
-        if (++v_st == v_stages) v_st = 0;
-      }
-    }
-    __syncwarp();
-  } else if (warp == 1) {
-    // ------------------------------------ MMA issuer ---------------------------------------
-    // One elected lane issues every tcgen05.mma of the CTA.  Under contention with the softmax warps of its SM
-    // sub-partition that lane retires about one instruction per 7 clocks, and before this loop was made lean (converged
-    // warp -> warp-uniform operands -> bare UTCHMMA; descriptors advanced by adds) its ~250 instructions per kv tile
-    // WERE the kernel's critical path (tools/attn_trace.py: 655 clocks to issue 4 MMAs + 2 commits).
-    // The kv tiles of all the CTA's Q tiles form one stream t = 0 .. T-1 (tile t: item t / nkv, kv tile t % nkv).
-    const bool leader = elect_one();
-    ATTN_TRACE_PTR(leader && p.trace && blockIdx.x == 3 && blockIdx.y == 2 && blockIdx.z == 1);
-    const bool bf = p.is_bf16 != 0;
-    const int ksteps_qk = p.d16 / 16, k_stages = p.k_stages, p_bufs = p.p_bufs, skv = p.Skv;
-    const int T = n_items * nkv;
-    const uint32_t tm_S = warp_uniform(tmem_base);
-    const uint32_t tm_Oa = tm_S + static_cast<uint32_t>(kSBufs * kKv), tm_Ob = tm_Oa + static_cast<uint32_t>(p.dpv);
-    const uint32_t bar0 = warp_uniform(smem_u32(sh));
-    const uint32_t a_k_full = bar0 + static_cast<uint32_t>(offsetof(AttnShared, k_full));
-    const uint32_t a_v_full = bar0 + static_cast<uint32_t>(offsetof(AttnShared, v_full));
-    const uint32_t a_s_full = bar0 + static_cast<uint32_t>(offsetof(AttnShared, s_full));
-    const uint32_t a_p_full = bar0 + static_cast<uint32_t>(offsetof(AttnShared, p_full));
-    const uint32_t a_o_full = bar0 + static_cast<uint32_t>(offsetof(AttnShared, o_full));
-    const uint32_t a_q_full = bar0 + static_cast<uint32_t>(offsetof(AttnShared, q_full));
-    const uint32_t a_q_empty = bar0 + static_cast<uint32_t>(offsetof(AttnShared, q_empty));
-    const uint32_t a_o_free = bar0 + static_cast<uint32_t>(offsetof(AttnShared, o_free));
-    // descriptor low words (address >> 4 | LBO field); the high word (SBO 1024, version, SWIZZLE_128B) is one constant
-    const uint32_t s0 = warp_uniform(smem_u32(sQ));
-    const uint32_t hi = sdesc_hi_sw128(1024);
-    const uint32_t q_lo0 = sdesc_lo(s0, 16);
-    const uint32_t q_all = static_cast<uint32_t>(p.q_bufs) * q_bytes;
-    const uint32_t p_lo0 = sdesc_lo(s0 + q_all, 16);
-    const uint32_t p_all = static_cast<uint32_t>(p.p_smem) * kPBytes;
-    const uint32_t k_lo0 = sdesc_lo(s0 + q_all + p_all, 16);
-    const uint32_t v_lo0 = sdesc_lo(s0 + q_all + p_all + static_cast<uint32_t>(k_stages) * kv_bytes,
-                                    kKvChunkBytes);  // V is consumed MN-major: LBO = distance between 64-wide chunks
-    const uint32_t kv_step = kv_bytes >> 4;
-    const uint32_t idesc_qk_full = make_idesc_f16(128, kKv, bf, false, false);
-    const uint32_t idesc_pv = make_idesc_f16(128, p.dpv, bf, false, true);  // B (= V) is MN-major
-    int qk_t = 0, qk_item = 0, qk_j = 0;  // resident mode, next Q.K: stream index, item (Q tile), kv tile
-    auto issue_qk = [&]() {  // resident mode: S[qk_t & 1] = Q_item K_j^T
-      const uint32_t q_sb = static_cast<uint32_t>(qk_t) & 1u;
-      const uint32_t qs = static_cast<uint32_t>(qk_item) & 1u;
-      const int nvalid = min(kKv, skv - qk_j * kKv);
-      ATTN_TRACE(11, qk_t);
-      if (qk_j == 0) mbar_wait_a(a_q_full + qs * 8u, (static_cast<uint32_t>(qk_item) >> 1) & 1u, 13);
-      const uint32_t kslot = static_cast<uint32_t>(qk_j);
-      const uint32_t k_lo = k_lo0 + kslot * kv_step;
-      mbar_wait_a(a_k_full + kslot * 8u, 0u, 14);  // loaded once per CTA
-      tc_fence_after();
-      ATTN_TRACE(12, qk_t);
-      if (leader) {
-        const uint32_t idesc = nvalid == kKv ? idesc_qk_full : make_idesc_f16(128, (nvalid + 15) & ~15, bf, false, false);
-        const uint32_t d_tmem = tm_S + q_sb * kKv;
-        const uint32_t q_lo = q_lo0 + qs * (q_bytes >> 4);
-        if (ksteps_qk == 3) {  // d = 40: the shape that dominates; straight-line issue
-          umma_f16_ss_lh(d_tmem, q_lo, hi, k_lo, hi, idesc, 0u);
-          umma_f16_ss_lh(d_tmem, q_lo + 2u, hi, k_lo + 2u, hi, idesc, 1u);
-          umma_f16_ss_lh(d_tmem, q_lo + 4u, hi, k_lo + 4u, hi, idesc, 1u);
-        } else {
-          for (int k = 0; k < ksteps_qk; ++k) {
-            const uint32_t ch = static_cast<uint32_t>(k) >> 2, in = (static_cast<uint32_t>(k) & 3u) * 2u;
-            umma_f16_ss_lh(d_tmem, q_lo + ch * (kQChunkBytes >> 4) + in, hi, k_lo + ch * (kKvChunkBytes >> 4) + in, hi,
-                           idesc, k != 0 ? 1u : 0u);
-          }
-        }
-        if (qk_j == nkv - 1) umma_commit_a(a_q_empty + qs * 8u);  // this Q buffer may be refilled
-        umma_commit_a(a_s_full + q_sb * 8u);
-      }
-      ATTN_TRACE(13, qk_t);
-      ++qk_t;
-      if (++qk_j == nkv) {
-        qk_j = 0;
-        ++qk_item;
-      }
-    };
-    if (!resident) {
-      // ---- ring mode: one Q tile, tiles t = 0 .. nkv-1.  Unrolled by six (the common period of the P ring of 3, the K
-      // ring of 3, the V ring of 2, the S pair and the p_full parity), so every slot address and barrier parity of a step
-      // is a constant: this thread's instruction count per tile bounds the kernel (see the header). ----
-      const int nvalid_last = skv - (nkv - 1) * kKv;
-      const bool p_tmem = p.p_tmem != 0;
-      const uint32_t idesc_qk_last = make_idesc_f16(128, (nvalid_last + 15) & ~15, bf, false, false);
-      auto qk = [&](int tile, uint32_t q_sb, uint32_t kslot) {  // leader only
-        const uint32_t idesc = tile == nkv - 1 ? idesc_qk_last : idesc_qk_full;
-        const uint32_t d_tmem = tm_S + q_sb * kKv;
-        const uint32_t k_lo = k_lo0 + kslot * kv_step;
-        if (ksteps_qk == 3) {  // d = 40: the shape that dominates; straight-line issue
-          umma_f16_ss_lh(d_tmem, q_lo0, hi, k_lo, hi, idesc, 0u);
-          umma_f16_ss_lh(d_tmem, q_lo0 + 2u, hi, k_lo + 2u, hi, idesc, 1u);
-          umma_f16_ss_lh(d_tmem, q_lo0 + 4u, hi, k_lo + 4u, hi, idesc, 1u);
-        } else {
-          for (int k = 0; k < ksteps_qk; ++k) {
-            const uint32_t ch = static_cast<uint32_t>(k) >> 2, in = (static_cast<uint32_t>(k) & 3u) * 2u;
-            umma_f16_ss_lh(d_tmem, q_lo0 + ch * (kQChunkBytes >> 4) + in, hi, k_lo + ch * (kKvChunkBytes >> 4) + in, hi,
-                           idesc, k != 0 ? 1u : 0u);
-          }
-        }
-        umma_commit_a(a_s_full + q_sb * 8u);
-      };
-      mbar_wait_a(a_q_full, 0u, 13);  // Q, K_0, K_1
-      tc_fence_after();
-      if (leader) {
-        qk(0, 0u, 0u);
-        if (nkv > 1) qk(1, 1u, 1u);
-      }
-      for (int t0 = 0; t0 < nkv; t0 += 6) {
+  auto load_kv = [&](int t) {  // tile t into slot t % stages (the slot is free)
+    const int s = t % p.stages;
+    mbar_arrive_expect_tx(&sh->kv_full[s], 2 * kKvBytes);
 #pragma unroll
-        for (int u = 0; u < 6; ++u) {
-          const int t = t0 + u;
-          if (t >= nkv) break;
-          ATTN_TRACE(7, t);
-          mbar_wait_a(a_p_full + static_cast<uint32_t>(u % 3) * 8u, static_cast<uint32_t>(u / 3), 15);  // P_t, K_{t+2}, V_t
-          tc_fence_after();
-          ATTN_TRACE(8, t);
-          if (leader && p_tmem) {
-            // P lives in S[t & 1]: P.V first, then Q.K of tile t+2 may overwrite the buffer (MMAs execute in issue order)
-            const uint32_t a_p = tm_S + static_cast<uint32_t>(u & 1) * kKv;
-            const uint32_t v_lo = v_lo0 + static_cast<uint32_t>(u & 1) * kv_step;
-            const uint32_t acc = t != 0 ? 1u : 0u;
-            const int ksteps_pv = (t != nkv - 1) ? 4 : ((nvalid_last + 15) & ~15) / 16;
-            umma_f16_ts_lh(tm_Oa, a_p + 0u, v_lo + 0u, hi, idesc_pv, acc);
-            if (ksteps_pv > 2) umma_f16_ts_lh(tm_Ob, a_p + 32u, v_lo + 256u, hi, idesc_pv, acc);
-            if (ksteps_pv > 1) umma_f16_ts_lh(tm_Oa, a_p + 8u, v_lo + 128u, hi, idesc_pv, 1u);
-            if (ksteps_pv > 3) umma_f16_ts_lh(tm_Ob, a_p + 40u, v_lo + 384u, hi, idesc_pv, 1u);
-            umma_commit_a(a_o_full + static_cast<uint32_t>(u % 3) * 8u);
-            if (t + 2 < nkv) qk(t + 2, static_cast<uint32_t>(u & 1), static_cast<uint32_t>((u + 2) % 3));
-            ATTN_TRACE(13, t + 2);
-          } else if (leader) {
-            // Q.K of tile t+2 first: S is what the softmax warps wait for next, O is not read until the end
-            if (t + 2 < nkv) qk(t + 2, static_cast<uint32_t>(u & 1), static_cast<uint32_t>((u + 2) % 3));
-            ATTN_TRACE(13, t + 2);
-            const uint32_t p_lo = p_lo0 + static_cast<uint32_t>(u % 3) * (kPBytes >> 4);
-            const uint32_t v_lo = v_lo0 + static_cast<uint32_t>(u & 1) * kv_step;
-            const uint32_t acc = t != 0 ? 1u : 0u;  // the first MMA into each accumulator overwrites it
-            if (t != nkv - 1 || nvalid_last == kKv) {
-              // k-step s reads P columns [16s, 16s+16) (2 descriptor units apart) and V rows [16s, 16s+16) (128 units
-              // apart); the two accumulators alternate so that consecutive MMAs never depend on each other
-              umma_f16_ss_lh(tm_Oa, p_lo + 0u, hi, v_lo + 0u, hi, idesc_pv, acc);
-              umma_f16_ss_lh(tm_Ob, p_lo + 4u, hi, v_lo + 256u, hi, idesc_pv, acc);
-              umma_f16_ss_lh(tm_Oa, p_lo + 2u, hi, v_lo + 128u, hi, idesc_pv, 1u);
-              umma_f16_ss_lh(tm_Ob, p_lo + 6u, hi, v_lo + 384u, hi, idesc_pv, 1u);
-            } else {
-              const int ksteps_pv = ((nvalid_last + 15) & ~15) / 16;
-              for (int k = 0; k < ksteps_pv; ++k)
-                umma_f16_ss_lh(k < 2 ? tm_Oa : tm_Ob, p_lo + 2u * k, hi, v_lo + 128u * k, hi, idesc_pv,
-                               (k & 1) == 0 ? acc : 1u);
-            }
-            umma_commit_a(a_o_full + static_cast<uint32_t>(u % 3) * 8u);
-          }
-          ATTN_TRACE(10, t);
-        }
-      }
-    } else {
-      for (int i = 0; i < kSBufs && i < T; ++i) issue_qk();
-      // ---- resident mode: K / V stay in shared memory, the tiles of all the CTA's Q tiles form one stream ----
-      int pb = 0, pv_item = 0, pv_j = 0;
-      uint32_t p_par = 0, p_lo = p_lo0;
-      for (int t = 0; t < T; ++t) {
-        const int nvalid = min(kKv, skv - pv_j * kKv);
-        ATTN_TRACE(7, t);
-        mbar_wait_a(a_p_full + static_cast<uint32_t>(pb) * 8u, p_par, 15);
-        ATTN_TRACE(8, t);
-        // ---- O_a (+)= P[:, 0:32] V[0:32, :],  O_b (+)= P[:, 32:64] V[32:64, :] ----
-        if (pv_j == 0 && pv_item > 0)  // the previous Q tile's epilogue has read the accumulators this P.V overwrites
-          mbar_wait_a(a_o_free, (static_cast<uint32_t>(pv_item) - 1u) & 1u, 21);
-        const uint32_t vslot = static_cast<uint32_t>(pv_j);
-        const uint32_t v_lo = v_lo0 + vslot * kv_step;
-        mbar_wait_a(a_v_full + vslot * 8u, 0u, 16);  // loaded once per CTA
-        tc_fence_after();
-        ATTN_TRACE(9, t);
-        if (leader) {
-          const uint32_t acc = pv_j != 0 ? 1u : 0u;  // the first MMA of a Q tile into each accumulator overwrites it
-          if (p.p_tmem) {
-            // P lives in the S buffer of this tile (TMEM): k-step s = columns [8s, 8s+8) of the half's 16 P columns
-            const uint32_t a_p = tm_S + (static_cast<uint32_t>(t) & 1u) * kKv;
-            const int ksteps_pv = ((nvalid + 15) & ~15) / 16;
-            umma_f16_ts_lh(tm_Oa, a_p + 0u, v_lo + 0u, hi, idesc_pv, acc);
-            if (ksteps_pv > 2) umma_f16_ts_lh(tm_Ob, a_p + 32u, v_lo + 256u, hi, idesc_pv, acc);
-            if (ksteps_pv > 1) umma_f16_ts_lh(tm_Oa, a_p + 8u, v_lo + 128u, hi, idesc_pv, 1u);
-            if (ksteps_pv > 3) umma_f16_ts_lh(tm_Ob, a_p + 40u, v_lo + 384u, hi, idesc_pv, 1u);
-          } else if (nvalid == kKv) {
-            // k-step s reads P columns [16s, 16s+16) (2 descriptor units apart) and V rows [16s, 16s+16) (128 units apart);
-            // the two accumulators alternate so that consecutive MMAs never depend on each other
-            umma_f16_ss_lh(tm_Oa, p_lo + 0u, hi, v_lo + 0u, hi, idesc_pv, acc);
-            umma_f16_ss_lh(tm_Ob, p_lo + 4u, hi, v_lo + 256u, hi, idesc_pv, acc);
-            umma_f16_ss_lh(tm_Oa, p_lo + 2u, hi, v_lo + 128u, hi, idesc_pv, 1u);
-            umma_f16_ss_lh(tm_Ob, p_lo + 6u, hi, v_lo + 384u, hi, idesc_pv, 1u);
-          } else {
-            const int ksteps_pv = ((nvalid + 15) & ~15) / 16;
-            for (int k = 0; k < ksteps_pv; ++k)
-              umma_f16_ss_lh(k < 2 ? tm_Oa : tm_Ob, p_lo + 2u * k, hi, v_lo + 128u * k, hi, idesc_pv,
-                             (k & 1) == 0 ? acc : 1u);
-          }
-          umma_commit_a(a_o_full + static_cast<uint32_t>(pb) * 8u);
-        }
-        ATTN_TRACE(10, t);
-        p_lo += kPBytes >> 4;
-        if (++pb == p_bufs) {
-          pb = 0;
-          p_par ^= 1u;
-          p_lo = p_lo0;
-        }
-        if (++pv_j == nkv) {
-          pv_j = 0;
-          ++pv_item;
-        }
-        // softmax t has released its S buffer (and P.V of this tile, which reads P from it, is already in the queue):
-        // refill it two tiles ahead
-        if (qk_t < T) issue_qk();
-      }
+    for (int c = 0; c < kChunks; ++c) {
+      tma_load_3d(sK + s * kKvBytes + c * kKvChunkBytes, &tmK, &sh->kv_full[s], col0 + c * 64, t * kKv, b);
+      tma_load_3d(sV + s * kKvBytes + c * kKvChunkBytes, &tmV, &sh->kv_full[s], col0 + c * 64, t * kKv, b);
     }
-    __syncwarp();
-  } else {
-    const bool sum_here = p.l_col < 0;
-    if (p.is_bf16) {
-      if (sum_here) softmax_warps<true, true>(p, sh, sP, tmem_base, warp, lane, first_qt, n_items, head, b, nkv);
-      else          softmax_warps<true, false>(p, sh, sP, tmem_base, warp, lane, first_qt, n_items, head, b, nkv);
-    } else {
-      if (sum_here) softmax_warps<false, true>(p, sh, sP, tmem_base, warp, lane, first_qt, n_items, head, b, nkv);
-      else          softmax_warps<false, false>(p, sh, sP, tmem_base, warp, lane, first_qt, n_items, head, b, nkv);
-    }
+  };
+  if (loader) {
+    mbar_arrive_expect_tx(&sh->q_full, kChunks * kQChunkBytes);
+#pragma unroll
+    for (int c = 0; c < kChunks; ++c) tma_load_3d(sQ + c * kQChunkBytes, &tmQ, &sh->q_full, col0 + c * 64, qt * kQTile, b);
+    for (int t = 0; t < p.stages && t < nkv; ++t) load_kv(t);
   }
 
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, static_cast<uint32_t>(p.tmem_cols));
+  const int colq = (lane & 3) * 2;  // accumulator columns 8g + colq, +1 of rows r0 (h = 0) and r0 + 8 (h = 1)
+  const uint32_t sQ_a = smem_u32(sQ) + static_cast<uint32_t>(wg) * 8192u;
+  const uint32_t sK_a = smem_u32(sK), sV_a = smem_u32(sV);
+  float o[kDv / 2];
+#pragma unroll
+  for (int i = 0; i < kDv / 2; ++i) o[i] = 0.f;
+  float m_run[2] = {-INFINITY, -INFINITY}, l_run[2] = {0.f, 0.f};
+  mbar_wait(&sh->q_full, 0);
+
+  for (int t = 0; t < nkv; ++t) {
+    // refill the slot of tile t-1 with tile t-1+stages once both warpgroups are done with it
+    if (loader && t > 0 && t - 1 + p.stages < nkv) {
+      const int s = (t - 1) % p.stages;
+      mbar_wait(&sh->kv_empty[s], static_cast<uint32_t>((t - 1) / p.stages) & 1u);
+      load_kv(t - 1 + p.stages);
+    }
+    const int s = t % p.stages;
+    mbar_wait(&sh->kv_full[s], static_cast<uint32_t>(t / p.stages) & 1u);
+
+    // S = Q K^T
+    float sacc[32];
+    const uint32_t k_a = sK_a + static_cast<uint32_t>(s) * kKvBytes;
+    wgmma_fence();
+    for (int ks = 0; ks < p.d16 / 16; ++ks) {
+      const uint32_t off = static_cast<uint32_t>(ks & 3) * 32u;  // k16 step inside the 128-byte swizzled row
+      Wgmma<64, kBf16>::ss(sacc, make_gdesc_sw128(sQ_a + static_cast<uint32_t>(ks >> 2) * kQChunkBytes + off, 16, 1024),
+                           make_gdesc_sw128(k_a + static_cast<uint32_t>(ks >> 2) * kKvChunkBytes + off, 16, 1024),
+                           ks != 0 ? 1u : 0u);
+    }
+    wgmma_commit();
+    wgmma_wait<0>();
+    reg_fence(sacc);
+
+    // online softmax (scaled logits in log2 units); kv columns >= Skv are masked
+    const int valid = p.Skv - t * kKv;
+    float mx[2] = {-INFINITY, -INFINITY};
+#pragma unroll
+    for (int g = 0; g < 8; ++g)
+#pragma unroll
+      for (int h = 0; h < 2; ++h)
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+          float& v = sacc[4 * g + 2 * h + e];
+          v = (8 * g + colq + e < valid) ? v * p.scale_log2 : -INFINITY;
+          mx[h] = fmaxf(mx[h], v);
+        }
+    float alpha[2];
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      mx[h] = fmaxf(mx[h], __shfl_xor_sync(0xffffffffu, mx[h], 1));
+      mx[h] = fmaxf(mx[h], __shfl_xor_sync(0xffffffffu, mx[h], 2));
+      const float m_new = fmaxf(m_run[h], mx[h]);  // finite: every kv tile has at least one valid column
+      alpha[h] = fast_exp2(m_run[h] - m_new);      // 2^(-inf) = 0 on the first tile
+      m_run[h] = m_new;
+      l_run[h] *= alpha[h];
+    }
+#pragma unroll
+    for (int i = 0; i < kDv / 2; ++i) o[i] *= alpha[(i >> 1) & 1];
+    uint32_t pa[4][4];  // P as the A fragments of the four k16 steps of P.V
+#pragma unroll
+    for (int g = 0; g < 8; ++g)
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const float p0 = fast_exp2(sacc[4 * g + 2 * h] - m_run[h]);
+        const float p1 = fast_exp2(sacc[4 * g + 2 * h + 1] - m_run[h]);
+        l_run[h] += p0 + p1;
+        pa[g >> 1][(g & 1) * 2 + h] = pack_h2<kBf16>(p0, p1);
+      }
+
+    // O += P V
+    const uint32_t v_a = sV_a + static_cast<uint32_t>(s) * kKvBytes;
+    reg_fence(o);
+    wgmma_fence();
+#pragma unroll
+    for (int j = 0; j < 4; ++j)
+      Wgmma<kDv, kBf16>::rs_tb(o, pa[j], make_gdesc_sw128(v_a + static_cast<uint32_t>(j) * 2048u, kKvChunkBytes, 1024), 1u);
+    wgmma_commit();
+    wgmma_wait<0>();
+    reg_fence(o);
+    if ((threadIdx.x & 127) == 0) mbar_arrive(&sh->kv_empty[s]);
+  }
+
+  // O / l -> global (rows < Sq, columns < d)
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    l_run[h] += __shfl_xor_sync(0xffffffffu, l_run[h], 1);
+    l_run[h] += __shfl_xor_sync(0xffffffffu, l_run[h], 2);
+  }
+  const int r0 = qt * kQTile + wg * 64 + (warp & 3) * 16 + (lane >> 2);
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    const int row = r0 + 8 * h;
+    if (row >= p.Sq) continue;
+    const float inv = 1.0f / l_run[h];
+    uint8_t* orow = static_cast<uint8_t*>(p.O) + ((static_cast<long long>(b) * p.Sq + row) * p.ldo +
+                                                  static_cast<long long>(head) * p.d) * 2;
+#pragma unroll
+    for (int g = 0; g < kDv / 8; ++g) {
+      const int col = 8 * g + colq;
+      if (col < p.d)
+        *reinterpret_cast<uint32_t*>(orow + col * 2) = pack_h2<kBf16>(o[4 * g + 2 * h] * inv, o[4 * g + 2 * h + 1] * inv);
+    }
   }
 }
 
 // ------------------------------------------------------------------------------------------------
-static long long* g_attn_trace = nullptr;
+typedef void (*AttnKernel)(CUtensorMap, CUtensorMap, CUtensorMap, AttnParams);
+
+static AttnKernel attn_kernel_for(int chunks, int is_bf16) {
+  switch (chunks * 2 + (is_bf16 ? 1 : 0)) {
+    case 2: return attention_tc_kernel<1, false>;
+    case 3: return attention_tc_kernel<1, true>;
+    case 4: return attention_tc_kernel<2, false>;
+    case 5: return attention_tc_kernel<2, true>;
+    case 6: return attention_tc_kernel<3, false>;
+    case 7: return attention_tc_kernel<3, true>;
+    default: return nullptr;
+  }
+}
+
 static int g_attn_max_smem = 0;
 static bool g_attn_dev_ready[64] = {};
 
@@ -864,9 +245,7 @@ int attention_tc(const void* Q, long long ldq, const void* K, long long ldk, con
                  long long ldo, int B, int heads, int Sq, int Skv, int d, int d_pad, float scale, int v_ones_col,
                  int is_bf16, cudaStream_t stream) {
   if (B <= 0 || heads <= 0 || Sq <= 0) return B200SD_OK;
-  // d_pad: the head pitch in Q / K / V.  A multiple of 16 (the P.V MMA's N); the shared-memory tiles stay whole 64-column
-  // chunks — a box that runs past its head reads the next head's first columns (never multiplied: Q.K^T stops at d16, P.V
-  // at d_pad) or, for the last head, the tensor map's zero fill.
+  // d_pad: the head pitch in Q / K / V, a multiple of 16
   if (Skv <= 0 || d <= 0 || d % 8 != 0 || d_pad % 16 != 0 || d_pad < d) return B200SD_ERR_INVALID;
   if (ldq % 8 || ldk % 8 || ldv % 8 || ldo % 8) return B200SD_ERR_INVALID;
   if ((reinterpret_cast<uintptr_t>(Q) | reinterpret_cast<uintptr_t>(K) | reinterpret_cast<uintptr_t>(V) |
@@ -875,6 +254,9 @@ int attention_tc(const void* Q, long long ldq, const void* K, long long ldk, con
   if (ldq < static_cast<long long>(heads) * d_pad || ldk < static_cast<long long>(heads) * d_pad ||
       ldv < static_cast<long long>(heads) * d_pad || ldo < static_cast<long long>(heads) * d)
     return B200SD_ERR_INVALID;
+  if (v_ones_col && d >= d_pad) return B200SD_ERR_INVALID;  // the ones column needs a free pad column
+  const int chunks = (d_pad + 63) / 64;
+  if (chunks > 3) return B200SD_ERR_UNSUPPORTED;
   {
     int dev = 0;
     if (cudaGetDevice(&dev) != cudaSuccess) return B200SD_ERR_CUDA;
@@ -883,8 +265,11 @@ int attention_tc(const void* Q, long long ldq, const void* K, long long ldk, con
       int smem = 0;
       if (cudaDeviceGetAttribute(&smem, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev) != cudaSuccess)
         return B200SD_ERR_CUDA;
-      if (cudaFuncSetAttribute(attention_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem) != cudaSuccess)
-        return B200SD_ERR_CUDA;
+      for (int c = 1; c <= 3; ++c)
+        for (int bf = 0; bf < 2; ++bf)
+          if (cudaFuncSetAttribute(attn_kernel_for(c, bf), cudaFuncAttributeMaxDynamicSharedMemorySize, smem) !=
+              cudaSuccess)
+            return B200SD_ERR_CUDA;
       g_attn_max_smem = smem;
       g_attn_dev_ready[dev] = true;
     }
@@ -892,69 +277,14 @@ int attention_tc(const void* Q, long long ldq, const void* K, long long ldk, con
   AttnParams p{};
   p.B = B; p.heads = heads; p.Sq = Sq; p.Skv = Skv; p.d = d; p.d_pad = d_pad;
   p.d16 = (d + 15) & ~15;
-  p.chunks = (d_pad + 63) / 64;
+  p.chunks = chunks;
   p.scale_log2 = scale * 1.4426950408889634f;
-  p.O = O; p.ldo = ldo; p.is_bf16 = is_bf16;
-  p.trace = g_attn_trace;
-  p.dpv = d_pad;
-  // TMEM: two S buffers + one accumulator per kv-tile half.  d_pad 64 -> 256 columns (two CTAs per SM), up to 192 -> 512
-  if (kSBufs * kKv + 2 * p.dpv > 512) return B200SD_ERR_UNSUPPORTED;
-  if (v_ones_col && d >= d_pad) return B200SD_ERR_INVALID;  // needs a free pad column
-  p.l_col = v_ones_col ? d : -1;
-  p.resc_cols = v_ones_col ? ((d + 1 + 15) & ~15) : p.d16;
-  p.tmem_cols = (kSBufs * kKv + 2 * p.dpv <= 256) ? 256 : 512;
+  p.O = O; p.ldo = ldo;
   const int nkv = (Skv + kKv - 1) / kKv;
-  p.num_q_tiles = (Sq + kQTile - 1) / kQTile;
-  const size_t kvt = static_cast<size_t>(p.chunks) * kKvChunkBytes;
-  const size_t qt = static_cast<size_t>(p.chunks) * kQChunkBytes;
-  static int e_res = -1;  // experiment knob: B200SD_ATTN_RESIDENT=0 disables the resident-K/V mode
-  if (e_res < 0) {
-    const char* e = std::getenv("B200SD_ATTN_RESIDENT");
-    e_res = e ? std::atoi(e) : 1;
-  }
-  static int e_ptmem = -1;  // B200SD_ATTN_PTMEM=0: P through shared memory (the earlier form) instead of TMEM
-  if (e_ptmem < 0) {
-    const char* e = std::getenv("B200SD_ATTN_PTMEM");
-    e_ptmem = e ? std::atoi(e) : 1;
-  }
-  p.p_tmem = e_ptmem != 0 ? 1 : 0;
-  const size_t p_atom = p.p_tmem ? 0 : kPBytes;   // shared memory per P buffer
-  p.resident = (nkv <= 2 && e_res != 0) ? 1 : 0;
-  if (p.resident && 1024 + 2 * qt + 2 * p_atom + 2 * static_cast<size_t>(nkv) * kvt + sizeof(AttnShared) + 64 >
-                        static_cast<size_t>(g_attn_max_smem))
-    p.resident = 0;  // d_pad = 192 with two kv tiles: two Q buffers do not fit, use the ring form
-  size_t smem;
-  if (p.resident) {
-    // Cross-attention (77 context tokens): K / V of a (batch, head) are two tiles — loaded once per CTA, which then walks
-    // several Q tiles (the next one prefetched into a second Q buffer).  Per-CTA start-up (launch, TMEM allocation,
-    // first loads) dominated the one-tile-per-CTA form: 7 us per CTA for 2 us of work.
-    p.q_bufs = 2;
-    p.p_bufs = 2;  // P.V(t) is issued before Q.K(t+2) in this mode: "S[t] ready" covers P.V of tile t-2
-    p.k_stages = nkv;
-    p.v_stages = nkv;
-    // Q tiles per CTA: as many as keep at least one full wave of CTAs (148) in the grid, at most 8
-    p.qpc = 1;
-    for (int c = 8; c > 1; c >>= 1) {
-      const long long ctas = static_cast<long long>((p.num_q_tiles + c - 1) / c) * heads * B;
-      if (c <= p.num_q_tiles && ctas >= 148) {
-        p.qpc = c;
-        break;
-      }
-    }
-    p.p_smem = p.p_tmem ? 0 : p.p_bufs;
-    smem = 1024 + 2 * qt + 2 * p_atom + 2 * static_cast<size_t>(nkv) * kvt + sizeof(AttnShared) + 64;
-  } else {
-    // Ring mode.  shared memory: Q + three P atoms (required by the Q.K-first issue order, see the header) + K ring of 3
-    // + V ring of 2: 104 KB for d_pad == 64 (two CTAs per SM), 219 KB for d_pad == 192.
-    p.q_bufs = 1;
-    p.qpc = 1;
-    p.p_bufs = 3;
-    p.p_smem = p.p_tmem ? 0 : p.p_bufs;
-    const size_t fixed = 1024 + qt + sizeof(AttnShared) + 64 + 3 * p_atom;
-    p.k_stages = 3;  // the producer's slot-reuse argument (see the kernel) is written for exactly this ring: K 3 / V 2 / P 3
-    p.v_stages = 2;
-    smem = fixed + static_cast<size_t>(p.k_stages + p.v_stages) * kvt;
-  }
+  const size_t qt = static_cast<size_t>(chunks) * kQChunkBytes;
+  const size_t kvt = 2 * static_cast<size_t>(chunks) * kKvChunkBytes;  // K and V of one slot
+  p.stages = nkv < kMaxStages ? nkv : kMaxStages;
+  const size_t smem = 1024 + qt + static_cast<size_t>(p.stages) * kvt + sizeof(AttnShared);
   if (smem > static_cast<size_t>(g_attn_max_smem)) return B200SD_ERR_UNSUPPORTED;
   CUtensorMap tmQ, tmK, tmV;
   const uint32_t es[3] = {1, 1, 1};
@@ -976,15 +306,15 @@ int attention_tc(const void* Q, long long ldq, const void* K, long long ldk, con
     const uint64_t st[2] = {static_cast<uint64_t>(ldv) * 2, static_cast<uint64_t>(ldv) * 2 * Skv};
     if ((rc = make_tmap_sw128(&tmV, V, 3, dims, st, kvbox, es)) != B200SD_OK) return rc;
   }
-  dim3 grid((p.num_q_tiles + p.qpc - 1) / p.qpc, heads, B);
-  launch_pdl(attention_tc_kernel, grid, dim3(kAttnThreads), smem, stream, tmQ, tmK, tmV, p);
+  dim3 grid((Sq + kQTile - 1) / kQTile, heads, B);
+  launch_pdl(attn_kernel_for(chunks, is_bf16), grid, dim3(kAttnThreads), smem, stream, tmQ, tmK, tmV, p);
   return cudaGetLastError() == cudaSuccess ? B200SD_OK : B200SD_ERR_CUDA;
 }
 
 }  // namespace b200sd
 
-// debug hook: device buffer of 16 * 64 int64 that CTA (3, 2, 1) of later attention launches fills with clock64 stamps
+// debug hook kept for ABI compatibility: the sm_90a attention kernel records no timeline, so the buffer is never written
 extern "C" int b200sd_debug_attention_trace(void* device_buffer) {
-  b200sd::g_attn_trace = static_cast<long long*>(device_buffer);
+  (void)device_buffer;
   return B200SD_OK;
 }

@@ -397,7 +397,7 @@ extern "C" int b200sd_upsample2x(const void* X, long long pitch_x, void* Y, long
     return B200SD_ERR_INVALID;
   const long long total = static_cast<long long>(NB) * 4 * H * W * (C / 8);
   long long blocks = (total + 255) / 256;
-  if (blocks > 148 * 16) blocks = 148 * 16;
+  if (blocks > kNumSms * 16) blocks = kNumSms * 16;
   launch_pdl(upsample2x_kernel, dim3(static_cast<int>(blocks)), dim3(256), 0, ST(stream), static_cast<const uint4*>(X), pitch_x / 8, static_cast<uint4*>(Y), pitch_y / 8, NB, H, W, C / 8);
   RET_LAUNCH();
 }
@@ -414,7 +414,7 @@ extern "C" int b200sd_softmax_rows(void* S, long long lds, int rows, int cols, f
 extern "C" int b200sd_silu(const void* X, void* Y, long long n, int dtype, void* stream) {
   if (n <= 0) return B200SD_OK;
   long long blocks = (n + 255) / 256;
-  if (blocks > 148 * 8) blocks = 148 * 8;
+  if (blocks > kNumSms * 8) blocks = kNumSms * 8;
   if (dtype == B200SD_BF16) silu_kernel<true><<<static_cast<int>(blocks), 256, 0, ST(stream)>>>(X, Y, n);
   else silu_kernel<false><<<static_cast<int>(blocks), 256, 0, ST(stream)>>>(X, Y, n);
   RET_LAUNCH();
@@ -444,7 +444,7 @@ extern "C" int b200sd_select_step(const float* table, long long row_len, const i
                                   void* stream) {
   if (row_len <= 0) return B200SD_OK;
   long long blocks = (row_len + 255) / 256;
-  if (blocks > 148) blocks = 148;
+  if (blocks > kNumSms) blocks = kNumSms;
   launch_pdl(select_step_kernel, dim3(static_cast<int>(blocks)), dim3(256), 0, ST(stream), table, row_len, step_counter, cur);
   RET_LAUNCH();
 }

@@ -1,6 +1,6 @@
-// gemm_conv_tc.cu — persistent warp-specialised tcgen05 GEMM / implicit-GEMM convolution for sm_100a.
+// gemm_conv_tc.cu — persistent warp-specialised wgmma GEMM / implicit-GEMM convolution for sm_90a.
 //
-//   D[M, N] = epilogue( A[M, K] * Wt[N, K]^T )          fp16 or bf16 operands, fp32 accumulation in TMEM
+//   D[M, N] = epilogue( A[M, K] * Wt[N, K]^T )          fp16 or bf16 operands, fp32 accumulation in registers
 //
 // mode GEMM : A is a row-major [M, K] matrix (row pitch lda), loaded by 2-D TMA tiles {64 x 128}.
 //             Covers every Linear layer and every 1x1 convolution of the UNet / VAE (NHWC activations).
@@ -10,21 +10,26 @@
 //             (dx - pad, dy - pad) — TMA's out-of-bounds zero fill is the convolution padding, and
 //             elementStrides = 2 gives the stride-2 Downsample.  Weights are packed [Cout][tap][Cin].
 //
-// Roles (320 threads): warp 0 = TMA producer, warp 1 = TMEM allocator + single-thread tcgen05.mma issuer,
-// warps 2..9 = epilogue, two groups of four warps (one warp per TMEM lane quarter) that take alternate 32-column
-// chunks of the accumulator:  TMEM -> registers -> (+bias, +residual, SiLU / GEGLU) -> fp16 -> a SWIZZLE_64B
-// staging tile in shared memory -> TMA store.  The residual tile arrives the same way (TMA load into a staging
-// tile, two chunks ahead), so ALL global traffic of the kernel is bulk, coalesced and asynchronous; out-of-range
-// rows (M tail, partial pixel boxes) are clipped / zero-filled by the tensor maps instead of predicated.
-// Two TMEM accumulators (columns 0 and 256) let tile i's epilogue overlap tile i+1's MMAs.
+// Roles (384 threads): warps 0-7 are two consumer warpgroups, warpgroup 2 is the TMA producer, which releases registers
+// to the consumers at run time (setmaxnreg 40 / 232).  ptxas still allocates against the 168-register launch budget of
+// 12 warps, so BN = 192 / 224 / 256 (96-128 accumulator registers) spill 64-304 bytes per thread: those widths are kept
+// for callers that pass an explicit block_n and are correct, but ops.pick_block_n never chooses them.  Warpgroup w owns rows
+// [64w, 64w+64) of the 128 x BN tile: it issues m64nBNk16 wgmma on the shared-memory stages (A and B K-major,
+// SWIZZLE_128B) and keeps the fp32 accumulator in registers.  The producer fills a ring of stages (A 16 KB + B BN x 128 B)
+// that runs ahead into the next tile while the consumers are in their epilogue.  Epilogue, in 32-column chunks:
+// registers -> (+bias, GEGLU, +residual, SiLU) -> fp16 -> a SWIZZLE_64B staging tile in shared memory -> one TMA store
+// of the whole 128-row box.  The residual arrives the same way (TMA load into a staging tile, two chunks ahead), so all
+// global traffic of the kernel is bulk and asynchronous; out-of-range rows (M tail, partial pixel boxes) are clipped /
+// zero-filled by the tensor maps instead of predicated.
 //
-// Upstream ops this kernel stands in for (not in /root/reference; reached from world.py:196 / worker.py:432):
-// ldm ResBlock conv3x3 / skip 1x1, Up/Downsample conv, SpatialTransformer proj_in/out, CrossAttention
-// to_q/k/v/out, FeedForward GEGLU + out, AutoencoderKL decoder convs (SURVEY.md §8 a-ext x1,x2,x5,x7,x8,x9,x11).
+// Upstream ops this kernel stands in for: ldm ResBlock conv3x3 / skip 1x1, Up/Downsample conv, SpatialTransformer
+// proj_in/out, CrossAttention to_q/k/v/out, FeedForward GEGLU + out, AutoencoderKL decoder convs
+// (SURVEY.md §8 a-ext x1,x2,x5,x7,x8,x9,x11).
 #include <math.h>
 #include <stddef.h>
 #include <stdlib.h>
 #include "tc_common.cuh"
+#include "wgmma.cuh"
 #include "b200sd_internal.h"
 #include "pdl.cuh"
 
@@ -32,15 +37,13 @@ namespace b200sd {
 
 constexpr int kBlockM = 128;
 constexpr int kBlockK = 64;   // 64 halfs = 128 B = one SWIZZLE_128B row
-constexpr int kUmmaK = 16;
-constexpr int kEpiWarps = 8;  // two groups of 4 warps
-constexpr int kGemmThreads = 64 + 32 * kEpiWarps;
+constexpr int kMmaK = 16;
+constexpr int kConsumerThreads = 256;                 // two warpgroups of 64 rows each
+constexpr int kGemmThreads = kConsumerThreads + 128;  // + the producer warpgroup (one thread issues the TMA loads)
 constexpr int kMaxStages = 8;
-constexpr int kTmemCols = 512;
-constexpr int kAccStride = 256;
 constexpr int kChunkCols = 32;
 constexpr uint32_t kStageTileBytes = kBlockM * kChunkCols * 2;  // 8 KB: 128 rows x 32 halfs, SWIZZLE_64B
-constexpr uint32_t kStagingBytes = 4 * kStageTileBytes;         // [group][buffer]
+constexpr uint32_t kATileBytes = kBlockM * kBlockK * 2;         // 16 KB
 
 struct GemmKernelParams {
   int M, N, K;
@@ -56,155 +59,37 @@ struct GemmKernelParams {
   int bias_group_rows;             // rows (output pixels) sharing one bias row; <= 0 -> single row
   int has_residual;
   int flags;                       // B200SD_EPI_*
-  int is_bf16;
-  int pair;                        // 1: launched as CTA pairs (tcgen05 cta_group::2, 256-row tiles)
-  int d_bufs;                      // output staging buffers per epilogue group (2, or 3 so a TMA store may still be
-                                   // reading its buffer while the next chunk is staged)
-  long long* trace;                // debug: clock64 timeline of CTA 0 ([32 events][64 tiles]), or null
 };
 
-// debug timeline (b200sd_debug_gemm_trace; build with -DB200SD_GEMM_TRACE_ENABLE=1, tools/gemm_trace.py): CTA 0 stamps, per
-// tile it processes, events of the producer lane, the MMA lane and thread 0 of each epilogue group.  Compiled out by default.
-#ifndef B200SD_GEMM_TRACE_ENABLE
-#define B200SD_GEMM_TRACE_ENABLE 0
-#endif
-#if B200SD_GEMM_TRACE_ENABLE
-#define GEMM_TRACE(cond, ev, j) \
-  do { if ((cond) && p.trace != nullptr && blockIdx.x == 0) p.trace[(ev) * 64 + ((j) & 63)] = clock64(); } while (0)
-#else
-#define GEMM_TRACE(cond, ev, j) do { } while (0)
-#endif
-
-struct __align__(16) GemmBarriers {
-  uint64_t full[kMaxStages];
-  uint64_t empty[kMaxStages];
-  uint64_t tmem_full[2];
-  uint64_t tmem_empty[2];
-  uint64_t res_full[2][2];  // [group][buffer]: residual staging tile landed
-  uint32_t tmem_base;
-  uint32_t pad[3];          // bias_s starts 16-byte aligned (float4 reads)
-  float bias_s[2][2][128];  // [group][value | GEGLU gate][chunk ordinal * 32 + column]: this tile's bias, staged per group
+struct __align__(8) GemmBarriers {
+  uint64_t full[kMaxStages];   // stage landed (TMA transaction bytes)
+  uint64_t empty[kMaxStages];  // stage consumed: one arrival per consumer warpgroup
+  uint64_t res_full[2];        // residual staging tile landed
 };
 
-static_assert(offsetof(GemmBarriers, bias_s) % 16 == 0, "bias_s must be 16-byte aligned");
-
-// gelu(x) = 0.5 x (1 + erf(x / sqrt 2)), erf by Abramowitz-Stegun 7.1.26 (|abs err| < 1.5e-7, far below the fp16
-// output rounding): two MUFU ops (rcp, ex2) + a degree-5 Horner chain instead of erff()'s branchy ~30 instructions.
-__device__ __forceinline__ float gelu_erf(float x) {
-  const float z = fabsf(x) * 0.70710678118654752440f;
-  const float t = __fdividef(1.0f, fmaf(0.3275911f, z, 1.0f));
-  float poly = fmaf(1.061405429f, t, -1.453152027f);
-  poly = fmaf(poly, t, 1.421413741f);
-  poly = fmaf(poly, t, -0.284496736f);
-  poly = fmaf(poly, t, 0.254829592f);
-  const float erf_abs = 1.0f - poly * t * __expf(-z * z);
-  return 0.5f * x * (1.0f + copysignf(erf_abs, x));
-}
-
-// The same GELU on two values at once with Blackwell's packed fp32 pipe (FMUL2 / FFMA2 / FADD2): the GEGLU epilogue is
-// bound by instruction issue (8 epilogue warps must evaluate 128 x 128 GELUs per tile in the ~2560 clocks its MMAs
-// take), and the packed form needs ~12 instead of ~22 instructions per element.
-struct F2 {
-  uint64_t v;
-};
-__device__ __forceinline__ F2 f2(float a, float b) {
-  F2 r;
-  asm("mov.b64 %0, {%1, %2};" : "=l"(r.v) : "f"(a), "f"(b));
-  return r;
-}
-__device__ __forceinline__ void f2_get(F2 x, float& a, float& b) { asm("mov.b64 {%0, %1}, %2;" : "=f"(a), "=f"(b) : "l"(x.v)); }
-__device__ __forceinline__ F2 f2_mul(F2 a, F2 b) {
-  F2 r;
-  asm("mul.rn.f32x2 %0, %1, %2;" : "=l"(r.v) : "l"(a.v), "l"(b.v));
-  return r;
-}
-__device__ __forceinline__ F2 f2_add(F2 a, F2 b) {
-  F2 r;
-  asm("add.rn.f32x2 %0, %1, %2;" : "=l"(r.v) : "l"(a.v), "l"(b.v));
-  return r;
-}
-__device__ __forceinline__ F2 f2_fma(F2 a, F2 b, F2 c) {
-  F2 r;
-  asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(r.v) : "l"(a.v), "l"(b.v), "l"(c.v));
-  return r;
-}
+// gelu(x) = 0.5 x (1 + erf(x / sqrt 2)), erf by Abramowitz-Stegun 7.1.28: erf(z) = 1 - (1 + a1 z + ... + a6 z^6)^-16 for
+// z >= 0, |error| < 3e-7 (gelu: 9e-7 absolute over [-12, 12], far below the fp16 output rounding): one MUFU op (the
+// reciprocal; the 16th power is four squarings).  An overflow of the 16th power (z > ~15) gives rcp(inf) = 0, i.e.
+// erf = 1, which is the right limit.
 __device__ __forceinline__ float rcp_approx(float x) {
   float y;
   asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
   return y;
 }
-// gelu on two values.  erf by Abramowitz-Stegun 7.1.28: erf(z) = 1 - (1 + a1 z + ... + a6 z^6)^-16 for z >= 0, |error| < 3e-7
-// (gelu: 9e-7 absolute over [-12, 12]): ONE MUFU op per element (the reciprocal; the 16th power is four packed squarings)
-// where 7.1.26 above needs two (rcp and ex2).  tools/gemm_trace.py, round 2: a GEGLU tile's epilogue took 6000 clocks against
-// 2400 for its MMAs at K = 320 — 32768 MUFU lane-operations per tile are 2048 clocks of the SM's 16-lane MUFU pipe on their
-// own, and the two-MUFU dependency chain kept the eight epilogue warps latency-bound on top.  An overflow of the 16th power
-// (z > ~15) gives rcp(inf) = 0, i.e. erf = 1, which is the right limit.
-__device__ __forceinline__ F2 gelu_erf2(F2 x) {
-  float x0, x1;
-  f2_get(x, x0, x1);
-  const F2 z = f2_mul(f2(fabsf(x0), fabsf(x1)), f2(0.70710678118654752440f, 0.70710678118654752440f));
-  F2 q = f2_fma(f2(0.0000430638f, 0.0000430638f), z, f2(0.0002765672f, 0.0002765672f));
-  q = f2_fma(q, z, f2(0.0001520143f, 0.0001520143f));
-  q = f2_fma(q, z, f2(0.0092705272f, 0.0092705272f));
-  q = f2_fma(q, z, f2(0.0422820123f, 0.0422820123f));
-  q = f2_fma(q, z, f2(0.0705230784f, 0.0705230784f));
-  q = f2_fma(q, z, f2(1.0f, 1.0f));
-  q = f2_mul(q, q);
-  q = f2_mul(q, q);
-  q = f2_mul(q, q);
-  q = f2_mul(q, q);
-  float q0, q1;
-  f2_get(q, q0, q1);
-  const float e0 = 1.0f - rcp_approx(q0), e1 = 1.0f - rcp_approx(q1);   // erf(|x| / sqrt 2)
-  const F2 h = f2_fma(f2(0.5f, 0.5f), f2(copysignf(e0, x0), copysignf(e1, x1)), f2(0.5f, 0.5f));
-  return f2_mul(x, h);
-}
-
-// The same GELU on kN pairs at once, written stage by stage: every stage is kN INDEPENDENT packed instructions, so the
-// dependent chain of one element (1 mul, 6 fma, 4 mul, rcp, 1 fma, 1 mul ~ 100+ clocks of latency) is overlapped kN-fold
-// whatever the instruction scheduler makes of it.  tools/gemm_trace.py, round 2: with the per-pair form above a 32-column
-// GEGLU chunk took 2400-2800 clocks — 16 pairs executed almost back to back, two warps per scheduler cannot hide that.
-template <int kN>
-__device__ __forceinline__ void gelu_erf2_batch(F2 (&x)[kN]) {
-  F2 z[kN], q[kN];
-#pragma unroll
-  for (int i = 0; i < kN; ++i) {
-    float x0, x1;
-    f2_get(x[i], x0, x1);
-    z[i] = f2_mul(f2(fabsf(x0), fabsf(x1)), f2(0.70710678118654752440f, 0.70710678118654752440f));
-  }
-#pragma unroll
-  for (int i = 0; i < kN; ++i) q[i] = f2_fma(f2(0.0000430638f, 0.0000430638f), z[i], f2(0.0002765672f, 0.0002765672f));
-#pragma unroll
-  for (int i = 0; i < kN; ++i) q[i] = f2_fma(q[i], z[i], f2(0.0001520143f, 0.0001520143f));
-#pragma unroll
-  for (int i = 0; i < kN; ++i) q[i] = f2_fma(q[i], z[i], f2(0.0092705272f, 0.0092705272f));
-#pragma unroll
-  for (int i = 0; i < kN; ++i) q[i] = f2_fma(q[i], z[i], f2(0.0422820123f, 0.0422820123f));
-#pragma unroll
-  for (int i = 0; i < kN; ++i) q[i] = f2_fma(q[i], z[i], f2(0.0705230784f, 0.0705230784f));
-#pragma unroll
-  for (int i = 0; i < kN; ++i) q[i] = f2_fma(q[i], z[i], f2(1.0f, 1.0f));
-#pragma unroll
-  for (int k = 0; k < 4; ++k) {
-#pragma unroll
-    for (int i = 0; i < kN; ++i) q[i] = f2_mul(q[i], q[i]);
-  }
-  float e0[kN], e1[kN];
-#pragma unroll
-  for (int i = 0; i < kN; ++i) {
-    float q0, q1;
-    f2_get(q[i], q0, q1);
-    e0[i] = rcp_approx(q0);
-    e1[i] = rcp_approx(q1);
-  }
-#pragma unroll
-  for (int i = 0; i < kN; ++i) {
-    float x0, x1;
-    f2_get(x[i], x0, x1);
-    const F2 h = f2_fma(f2(0.5f, 0.5f), f2(copysignf(1.0f - e0[i], x0), copysignf(1.0f - e1[i], x1)), f2(0.5f, 0.5f));
-    x[i] = f2_mul(x[i], h);
-  }
+__device__ __forceinline__ float gelu_erf(float x) {
+  const float z = __fmul_rn(fabsf(x), 0.70710678118654752440f);
+  float q = __fmaf_rn(0.0000430638f, z, 0.0002765672f);
+  q = __fmaf_rn(q, z, 0.0001520143f);
+  q = __fmaf_rn(q, z, 0.0092705272f);
+  q = __fmaf_rn(q, z, 0.0422820123f);
+  q = __fmaf_rn(q, z, 0.0705230784f);
+  q = __fmaf_rn(q, z, 1.0f);
+  q = __fmul_rn(q, q);
+  q = __fmul_rn(q, q);
+  q = __fmul_rn(q, q);
+  q = __fmul_rn(q, q);
+  const float h = __fmaf_rn(0.5f, copysignf(1.0f - rcp_approx(q), x), 0.5f);
+  return __fmul_rn(x, h);
 }
 
 template <bool kBf16>
@@ -226,8 +111,8 @@ __device__ __forceinline__ float2 unpack2(uint32_t u) {
   }
 }
 
-__device__ __forceinline__ void group_bar_sync(int group) {  // named barriers 1, 2: the 128 threads of one group
-  asm volatile("bar.sync %0, 128;" ::"r"(group + 1) : "memory");
+__device__ __forceinline__ void consumer_bar_sync() {  // named barrier 1: the 256 consumer threads
+  asm volatile("bar.sync 1, %0;" ::"n"(kConsumerThreads) : "memory");
 }
 
 struct TileCoord {
@@ -246,308 +131,73 @@ __device__ __forceinline__ TileCoord tile_coord(const GemmKernelParams& p, int m
   return t;
 }
 
-// One epilogue group's share of a tile.  `uses` counts how often each residual buffer of this group has been
-// filled so far (mbarrier phase bookkeeping, identical in all 128 threads).  `chunk_count` is the number of chunks this
-// group has staged since the kernel started: the two staging buffers alternate ACROSS tiles, never per tile — the TMA
-// store of a tile's last chunk may still be reading its buffer when the next tile's first chunk is written, and only
-// the buffer of the store before that is known to be drained (bulk_wait_read precedes every store).
-// What one epilogue group needs to turn 32 fp32 accumulator columns into a stored output chunk.
-struct EpiCtx {
-  const GemmKernelParams* p;
-  const CUtensorMap* tmD;
-  const CUtensorMap* tmR;
-  GemmBarriers* bars;
-  uint8_t* my_d;   // this group's output staging buffers
-  uint8_t* my_r;   // this group's residual staging buffers
-  TileCoord tc;
-  int n_tile, out_bn, nchunks, group, r;
-  bool leader;
-  uint32_t base;   // chunks this group had staged before this tile (residual buffer parity)
-};
-
-__device__ __forceinline__ void load_residual(const EpiCtx& e, int buf, int c) {  // leader only
-  const GemmKernelParams& p = *e.p;
-  mbar_arrive_expect_tx(&e.bars->res_full[e.group][buf], p.d_bytes);
-  const int col = e.n_tile * e.out_bn + c * kChunkCols;
-  if (p.mode == 0) tma_load_2d(e.my_r + buf * kStageTileBytes, e.tmR, &e.bars->res_full[e.group][buf], col, e.tc.c1);
-  else tma_load_4d(e.my_r + buf * kStageTileBytes, e.tmR, &e.bars->res_full[e.group][buf], col, e.tc.c1, e.tc.c2, e.tc.c3);
+// global output row of tile row r (0 when r lies outside the problem: only used to pick a per-image bias row)
+__device__ __forceinline__ long long tile_row(const GemmKernelParams& p, const TileCoord& tc, int m_tile, int r) {
+  if (p.mode == 0) {
+    const long long row = static_cast<long long>(m_tile) * kBlockM + r;
+    return row < p.M ? row : 0;
+  }
+  const int x = tc.c1 + r % p.bw, y = tc.c2 + (r / p.bw) % p.bh, n = tc.c3 + r / (p.bw * p.bh);
+  return (x < p.W && y < p.H && n < p.NB && r < p.bw * p.bh * p.bn) ? (static_cast<long long>(n) * p.H + y) * p.W + x : 0;
 }
 
-// f[32] (bias / GEGLU already applied) -> + residual -> SiLU -> fp16 -> swizzled staging tile -> TMA store of chunk c
-template <bool kBf16>
-__device__ __forceinline__ void finish_chunk(const EpiCtx& e, float (&f)[32], int c, uint32_t ci, uint32_t (&uses)[2],
-                                             uint32_t& d_slot) {
-  const GemmKernelParams& p = *e.p;
-  const int buf = static_cast<int>((e.base + ci) & 1u);
-  const int r = e.r;
-  if (p.has_residual) {
-    mbar_wait(&e.bars->res_full[e.group][buf], uses[buf] & 1u, 5);
-    uses[buf]++;
-    const uint8_t* rt = e.my_r + buf * kStageTileBytes;
-#pragma unroll
-    for (int q = 0; q < 4; ++q) {
-      const uint4 rv = *reinterpret_cast<const uint4*>(rt + sw64_offset(r, q));
-      const uint32_t w[4] = {rv.x, rv.y, rv.z, rv.w};
-#pragma unroll
-      for (int k = 0; k < 4; ++k) {
-        const float2 t = unpack2<kBf16>(w[k]);
-        f[q * 8 + k * 2] += t.x;
-        f[q * 8 + k * 2 + 1] += t.y;
-      }
-    }
-  }
-  if (p.flags & B200SD_EPI_SILU) {
-#pragma unroll
-    for (int j = 0; j < 32; ++j) f[j] = __fdividef(f[j], 1.0f + __expf(-f[j]));
-  }
-  uint8_t* dt = e.my_d + d_slot * kStageTileBytes;
-#pragma unroll
-  for (int q = 0; q < 4; ++q) {
-    uint4 o;
-    o.x = pack2<kBf16>(f[q * 8 + 0], f[q * 8 + 1]);
-    o.y = pack2<kBf16>(f[q * 8 + 2], f[q * 8 + 3]);
-    o.z = pack2<kBf16>(f[q * 8 + 4], f[q * 8 + 5]);
-    o.w = pack2<kBf16>(f[q * 8 + 6], f[q * 8 + 7]);
-    *reinterpret_cast<uint4*>(dt + sw64_offset(r, q)) = o;
-  }
-  fence_proxy_async_smem();          // my staging writes (and residual reads) -> visible / ordered for the async proxy
-  // before chunk i+1 is staged into the buffer after this one, the store that last read THAT buffer must be done:
-  // with two buffers that is the previous store (wait for all), with three the one before it (one may stay in flight)
-  if (e.leader) {
-    if (p.d_bufs == 3) bulk_wait_read<1>();
-    else bulk_wait_read<0>();
-  }
-  group_bar_sync(e.group);
-  if (e.leader) {
-    const int col = e.n_tile * e.out_bn + c * kChunkCols;
-    if (p.mode == 0) tma_store_2d(e.tmD, dt, col, e.tc.c1);
-    else tma_store_4d(e.tmD, dt, col, e.tc.c1, e.tc.c2, e.tc.c3);
-    bulk_commit();
-    if (p.has_residual && c + 4 < e.nchunks) load_residual(e, buf, c + 4);  // everyone is past reading this buffer
-  }
-  if (++d_slot == static_cast<uint32_t>(p.d_bufs)) d_slot = 0;
+__device__ __forceinline__ void load_residual(const GemmKernelParams& p, const CUtensorMap* tmR, GemmBarriers* bars,
+                                              uint8_t* stage_r, const TileCoord& tc, int n_tile, int out_bn, int c) {
+  const int buf = c & 1;
+  mbar_arrive_expect_tx(&bars->res_full[buf], p.d_bytes);
+  const int col = n_tile * out_bn + c * kChunkCols;
+  uint8_t* dst = stage_r + buf * kStageTileBytes;
+  if (p.mode == 0) tma_load_2d(dst, tmR, &bars->res_full[buf], col, tc.c1);
+  else tma_load_4d(dst, tmR, &bars->res_full[buf], col, tc.c1, tc.c2, tc.c3);
 }
 
-// One epilogue group's share of a tile.  `uses` counts how often each residual buffer of this group has been
-// filled so far (mbarrier phase bookkeeping, identical in all 128 threads).  `chunk_count` is the number of chunks this
-// group has staged since the kernel started: the two staging buffers alternate ACROSS tiles, never per tile — the TMA
-// store of a tile's last chunk may still be reading its buffer when the next tile's first chunk is written, and only
-// the buffer of the store before that is known to be drained (bulk_wait_read precedes every store).
-template <bool kBf16>
-__device__ __forceinline__ void epilogue_tile(const GemmKernelParams& p, const CUtensorMap* tmD, const CUtensorMap* tmR,
-                                              GemmBarriers* bars, uint8_t* stage_d, uint8_t* stage_r,
-                                              uint64_t* tmem_full_bar, uint32_t full_parity, uint32_t tmem_acc,
-                                              int m_tile, int n_tile, int quarter, int group, int lane,
-                                              uint32_t (&uses)[2], uint32_t& chunk_count, uint32_t& d_slot, int tile_it) {
-  const int r = quarter * 32 + lane;  // row of the tile == TMEM lane
-  const bool geglu = (p.flags & B200SD_EPI_GEGLU) != 0;
-  EpiCtx e;
-  e.p = &p; e.tmD = tmD; e.tmR = tmR; e.bars = bars;
-  e.my_d = stage_d + group * p.d_bufs * kStageTileBytes;
-  e.my_r = stage_r + group * 2 * kStageTileBytes;
-  e.tc = tile_coord(p, m_tile);
-  e.n_tile = n_tile;
-  e.out_bn = geglu ? p.block_n / 2 : p.block_n;
-  e.nchunks = e.out_bn / kChunkCols;
-  e.group = group; e.r = r;
-  e.leader = (quarter == ((2 + 4 * group) & 3)) && lane == 0;  // lane 0 of the group's first warp
-  e.base = chunk_count;
-  const int out_bn = e.out_bn, nchunks = e.nchunks;
-  const uint32_t taddr_row = tmem_acc + (static_cast<uint32_t>(quarter * 32) << 16);
-
-  // per-row bias group (per-image bias): needs the global output row of this thread
-  const float* bias_row = p.bias;
-  if (p.bias != nullptr && p.bias_group_rows > 0) {
-    long long row;
-    if (p.mode == 0) {
-      row = static_cast<long long>(m_tile) * kBlockM + r;
-      if (row >= p.M) row = 0;
-    } else {
-      const int x = e.tc.c1 + r % p.bw, y = e.tc.c2 + (r / p.bw) % p.bh, n = e.tc.c3 + r / (p.bw * p.bh);
-      row = (x < p.W && y < p.H && n < p.NB && r < p.bw * p.bh * p.bn) ? (static_cast<long long>(n) * p.H + y) * p.W + x : 0;
-    }
-    bias_row = p.bias + (row / p.bias_group_rows) * p.N;
-  }
-
-  if (p.has_residual && e.leader) {  // two chunks ahead; the buffers are free (last tile's barriers passed)
-    if (group < nchunks) load_residual(e, e.base & 1u, group);
-    if (group + 2 < nchunks) load_residual(e, (e.base + 1u) & 1u, group + 2);
-  }
-  // One bias row for the whole tile (everything but the per-image conv1 biases): the group's 128 threads fetch the <= 128
-  // floats its chunks need with ONE coalesced load each while the tile's MMAs are still running, and the chunk loop reads
-  // them back as shared-memory broadcasts.  (ncu, round 1: the per-chunk __ldg of the bias was the epilogue's largest
-  // long-scoreboard stall, 6-10 % of the kernel's samples.)  The previous tile's reads are behind the group barrier that
-  // ended its last chunk.
-  const bool bias_staged = p.bias != nullptr && p.bias_group_rows <= 0;
-  float* bs_v = bars->bias_s[group][0];
-  float* bs_g = bars->bias_s[group][1];
-  if (bias_staged) {
-    const int k = r >> 5, j = r & 31, c = group + 2 * k;
-    if (c < nchunks) {
-      const int col = n_tile * p.block_n + c * kChunkCols + j;
-      bs_v[r] = __ldg(p.bias + col);
-      if (geglu) bs_g[r] = __ldg(p.bias + col + out_bn);
-    }
-    group_bar_sync(group);
-  }
-  [[maybe_unused]] const bool tracer = e.leader;  // one thread per epilogue group; events 8.. (group 0), 20.. (group 1)
-  [[maybe_unused]] const int ev0 = 8 + 12 * group;
-  GEMM_TRACE(tracer, ev0 + 0, tile_it);           // epilogue: waiting for the accumulator
-  mbar_wait(tmem_full_bar, full_parity, 4);
-  tc_fence_after();
-  GEMM_TRACE(tracer, ev0 + 1, tile_it);           // epilogue: accumulator complete
-
-  // f += this tile's bias for the 32 columns of chunk (c, ordinal ci)
-  auto add_bias = [&](float (&f)[32], int c, uint32_t ci) {
-    if (bias_staged) {
-#pragma unroll
-      for (int j = 0; j < 32; j += 4) {
-        const float4 b = *reinterpret_cast<const float4*>(bs_v + ci * 32 + j);
-        f[j] += b.x; f[j + 1] += b.y; f[j + 2] += b.z; f[j + 3] += b.w;
-      }
-    } else if (bias_row) {
-      const int col_in = n_tile * p.block_n + c * kChunkCols;  // column in the [N] space of the GEMM (bias index)
-#pragma unroll
-      for (int j = 0; j < 32; j += 4) {
-        const float4 b = __ldg(reinterpret_cast<const float4*>(bias_row + col_in + j));
-        f[j] += b.x; f[j + 1] += b.y; f[j + 2] += b.z; f[j + 3] += b.w;
-      }
-    }
-  };
-
-  uint32_t ci = 0;
-  if (geglu) {
-    // value and gate columns of a chunk are loaded together (one wait); the chunk is bound by the GELU arithmetic
-    for (int c = group; c < nchunks; c += 2, ++ci) {
-      uint32_t v[32], g[32];
-      tmem_ld_x32(taddr_row + c * kChunkCols, v);
-      tmem_ld_x32(taddr_row + out_bn + c * kChunkCols, g);
-      tmem_ld_wait();
-      GEMM_TRACE(tracer && ci < 4, ev0 + 2 + 2 * ci, tile_it);   // chunk ci: accumulator columns in registers
-      float f[32];
-#pragma unroll
-      for (int j = 0; j < 32; ++j) f[j] = __uint_as_float(v[j]);
-      add_bias(f, c, ci);
-      const int gcol = n_tile * p.block_n + c * kChunkCols + out_bn;
-#pragma unroll
-      for (int hb = 0; hb < 32; hb += 16) {   // two batches of 8 pairs: gate + bias -> gelu -> * value
-        F2 x[8];
-#pragma unroll
-        for (int j = 0; j < 16; j += 4) {
-          float4 b = make_float4(0.f, 0.f, 0.f, 0.f);
-          if (bias_staged) b = *reinterpret_cast<const float4*>(bs_g + ci * 32 + hb + j);
-          else if (bias_row) b = __ldg(reinterpret_cast<const float4*>(bias_row + gcol + hb + j));
-          x[j / 2] = f2_add(f2(__uint_as_float(g[hb + j]), __uint_as_float(g[hb + j + 1])), f2(b.x, b.y));
-          x[j / 2 + 1] = f2_add(f2(__uint_as_float(g[hb + j + 2]), __uint_as_float(g[hb + j + 3])), f2(b.z, b.w));
-        }
-        gelu_erf2_batch<8>(x);
-#pragma unroll
-        for (int i = 0; i < 8; ++i) {
-          const F2 y = f2_mul(f2(f[hb + 2 * i], f[hb + 2 * i + 1]), x[i]);
-          f2_get(y, f[hb + 2 * i], f[hb + 2 * i + 1]);
-        }
-      }
-      finish_chunk<kBf16>(e, f, c, ci, uses, d_slot);
-      GEMM_TRACE(tracer && ci < 4, ev0 + 3 + 2 * ci, tile_it);   // chunk ci: staged, group barrier passed
-    }
-  } else {
-    // (A software-pipelined form — the next chunk's TMEM load in flight while this one is processed, which would hide ~420
-    // of a chunk's ~1050 clocks on K = 320 tiles, tools/gemm_trace.py — needs two 32-register arrays alive across the
-    // chunk body; at this kernel's 168-register ceiling (10 warps: three share one sub-partition's file) ptxas spills
-    // them, and a spilled in-flight tcgen05.ld destination is a correctness hazard, not just a slow-down.  Not shipped.)
-    for (int c = group; c < nchunks; c += 2, ++ci) {
-      uint32_t v[32];
-      tmem_ld_x32(taddr_row + c * kChunkCols, v);
-      tmem_ld_wait();
-      GEMM_TRACE(tracer && ci < 4, ev0 + 2 + 2 * ci, tile_it);   // chunk ci: accumulator columns in registers
-      float f[32];
-#pragma unroll
-      for (int j = 0; j < 32; ++j) f[j] = __uint_as_float(v[j]);
-      add_bias(f, c, ci);
-      finish_chunk<kBf16>(e, f, c, ci, uses, d_slot);
-      GEMM_TRACE(tracer && ci < 4, ev0 + 3 + 2 * ci, tile_it);   // chunk ci: staged, group barrier passed
-    }
-  }
-  chunk_count = e.base + ci;
-}
-
-// kPair = false: one CTA per tile (M = 128).
-// kPair = true : launched as clusters of two CTAs; the pair computes a 256 x block_n tile with tcgen05 cta_group::2.
-//   CTA `rank` owns output rows [128*rank, 128*rank+128) of the pair tile (its own A rows, accumulator and epilogue)
-//   and stages B rows [rank*bn/2, (rank+1)*bn/2).  Only the leader (rank 0) issues MMAs; the `full` barriers that
-//   gate them live in the leader and collect the TMA bytes of both CTAs; commits are multicast to both CTAs.
-template <bool kPair>
+template <int BN, bool kBf16>
 __global__ void __launch_bounds__(kGemmThreads, 1)
 gemm_conv_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                     const __grid_constant__ CUtensorMap tmD, const __grid_constant__ CUtensorMap tmR,
                     const GemmKernelParams p) {
+  constexpr uint32_t kStageBytes = kATileBytes + BN * 128u;
   extern __shared__ uint8_t smem_raw[];
   // SWIZZLE_128B tiles need 1024-byte alignment.
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  const int bn_local = kPair ? p.block_n / 2 : p.block_n;  // B rows staged by this CTA
-  const uint32_t stage_bytes = 16384u + static_cast<uint32_t>(bn_local) * 128u;
-  uint8_t* stage_d = smem + static_cast<size_t>(p.num_stages) * stage_bytes;
-  uint8_t* stage_r = stage_d + static_cast<size_t>(p.d_bufs) * 2 * kStageTileBytes;
-  GemmBarriers* bars = reinterpret_cast<GemmBarriers*>(stage_r + (p.has_residual ? kStagingBytes : 0));
+  uint8_t* stage_d = smem + static_cast<size_t>(p.num_stages) * kStageBytes;  // 2 output staging tiles
+  uint8_t* stage_r = stage_d + 2 * kStageTileBytes;                            // 2 residual staging tiles (if any)
+  GemmBarriers* bars = reinterpret_cast<GemmBarriers*>(stage_r + (p.has_residual ? 2 * kStageTileBytes : 0));
 
   pdl_trigger();  // the next kernel of the chain may start its prologue as SMs free up (pdl.cuh)
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
-  const int rank = kPair ? static_cast<int>(cluster_ctarank()) : 0;
-  // work items: (m_tile or m_pair, n_tile); a pair covers m_tiles 2*m_pair and 2*m_pair + 1 (the second may be a
-  // phantom beyond the problem: its loads are zero-filled and its stores clipped by the tensor maps)
-  const int m_items = kPair ? (p.num_m_tiles + 1) / 2 : p.num_m_tiles;
-  const int num_items = m_items * p.num_n_tiles;
-  const int first_item = kPair ? static_cast<int>(blockIdx.x >> 1) : static_cast<int>(blockIdx.x);
-  const int item_step = kPair ? static_cast<int>(gridDim.x >> 1) : static_cast<int>(gridDim.x);
+  const int num_items = p.num_m_tiles * p.num_n_tiles;
 
-  if (warp == 0 && lane == 0) {
+  if (threadIdx.x == kConsumerThreads) {
     tma_prefetch_desc(&tmA);
     tma_prefetch_desc(&tmB);
     tma_prefetch_desc(&tmD);
     if (p.has_residual) tma_prefetch_desc(&tmR);
     for (int s = 0; s < p.num_stages; ++s) {
       mbar_init(&bars->full[s], 1);
-      mbar_init(&bars->empty[s], 1);
+      mbar_init(&bars->empty[s], kConsumerThreads / 128);
     }
-    for (int a = 0; a < 2; ++a) {
-      mbar_init(&bars->tmem_full[a], 1);
-      mbar_init(&bars->tmem_empty[a], (kPair ? 2 : 1) * kEpiWarps);  // one arrival per epilogue warp (both CTAs')
-      mbar_init(&bars->res_full[a][0], 1);
-      mbar_init(&bars->res_full[a][1], 1);
-    }
+    mbar_init(&bars->res_full[0], 1);
+    mbar_init(&bars->res_full[1], 1);
     fence_mbar_init();
   }
-  if (warp == 1) {
-    if constexpr (kPair) tmem_alloc_pair(&bars->tmem_base, kTmemCols);
-    else tmem_alloc(&bars->tmem_base, kTmemCols);
-  }
-  tc_fence_before();
-  if constexpr (kPair) cluster_sync_all();  // the peer's barriers must be initialised before anything signals them
-  else __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = bars->tmem_base;
+  __syncthreads();
   pdl_wait();  // prologue done; from here on the kernel reads what its predecessors wrote
 
-  if (warp == 0) {
-    // ------------------------------- TMA producer -------------------------------
-    // Converged warp, one elected issuing lane (see the MMA issuer below); the (tap, channel-block) position of the
-    // conv K loop is advanced by counters — a division per k-block on this single thread was as slow as the MMAs.
-    {
-      const bool leader = elect_one();
-      const uint32_t bar0 = warp_uniform(smem_u32(bars));
-      const uint32_t a_full = bar0 + static_cast<uint32_t>(offsetof(GemmBarriers, full));
-      const uint32_t a_empty = bar0 + static_cast<uint32_t>(offsetof(GemmBarriers, empty));
+  if (warp >= kConsumerThreads / 32) {
+    // ------------------------------- TMA producer (one thread) -------------------------------
+    // The (tap, channel-block) position of the conv K loop is advanced by counters, not divisions.
+    setmaxnreg_dec<40>();
+    if (threadIdx.x == kConsumerThreads) {
       const int nkb = p.num_k_blocks, nstages = p.num_stages, cblocks = p.cblocks;
       const bool conv = p.mode == 1, taps9 = p.taps == 9;
-      const uint32_t tx_bytes = (kPair ? 2u : 1u) * (p.a_bytes + p.b_bytes);
+      const uint32_t tx_bytes = p.a_bytes + p.b_bytes;
       int stage = 0;
       uint32_t phase = 0;
-      int pit = 0;
-      for (int item = first_item; item < num_items; item += item_step, ++pit) {
+      for (int item = blockIdx.x; item < num_items; item += gridDim.x) {
         const int n_tile = item % p.num_n_tiles;
-        const int m_tile = kPair ? 2 * (item / p.num_n_tiles) + rank : item / p.num_n_tiles;
-        GEMM_TRACE(leader, 0, pit);   // producer: tile start
+        const int m_tile = item / p.num_n_tiles;
         int cx = 0, cy = 0, cn = 0;
         if (conv) {
           const int tx = m_tile % p.tiles_x;
@@ -556,146 +206,181 @@ gemm_conv_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_consta
           cx = tx * p.bw * p.stride - p.pad;
           cy = ty * p.bh * p.stride - p.pad;
         }
-        const int b_row = n_tile * p.block_n + (kPair ? rank * bn_local : 0);
+        const int b_row = n_tile * BN;
         const int a_row = m_tile * kBlockM;
         int cb = 0, dx = 0, dy = 0;  // conv: channel block within the tap, tap offsets
         for (int kb = 0; kb < nkb; ++kb) {
-          mbar_wait_a(a_empty + static_cast<uint32_t>(stage) * 8u, phase ^ 1u, 1);
-          if (leader) {
-            uint8_t* sA = smem + static_cast<size_t>(stage) * stage_bytes;
-            uint8_t* sB = sA + 16384;
-            uint64_t* full_bar = &bars->full[stage];
-            if constexpr (kPair) {
-              // both CTAs' bytes land on the LEADER's barrier; only the leader arms it (for the bytes of both)
-              const uint32_t lead_bar = mapa_u32(a_full + static_cast<uint32_t>(stage) * 8u, 0);
-              if (rank == 0) mbar_arrive_expect_tx(full_bar, tx_bytes);
-              if (!conv) tma_load_2d_pair(sA, &tmA, lead_bar, kb * kBlockK, a_row);
-              else tma_load_4d_pair(sA, &tmA, lead_bar, cb * kBlockK, cx + dx, cy + dy, cn);
-              tma_load_2d_pair(sB, &tmB, lead_bar, kb * kBlockK, b_row);
-            } else {
-              mbar_arrive_expect_tx(full_bar, tx_bytes);
-              if (!conv) tma_load_2d(sA, &tmA, full_bar, kb * kBlockK, a_row);
-              else tma_load_4d(sA, &tmA, full_bar, cb * kBlockK, cx + dx, cy + dy, cn);
-              tma_load_2d(sB, &tmB, full_bar, kb * kBlockK, b_row);
-            }
-          }
+          mbar_wait(&bars->empty[stage], phase ^ 1u);
+          uint8_t* sA = smem + static_cast<size_t>(stage) * kStageBytes;
+          uint8_t* sB = sA + kATileBytes;
+          uint64_t* full_bar = &bars->full[stage];
+          mbar_arrive_expect_tx(full_bar, tx_bytes);
+          if (!conv) tma_load_2d(sA, &tmA, full_bar, kb * kBlockK, a_row);
+          else tma_load_4d(sA, &tmA, full_bar, cb * kBlockK, cx + dx, cy + dy, cn);
+          tma_load_2d(sB, &tmB, full_bar, kb * kBlockK, b_row);
           if (++cb == cblocks) {  // next tap (1x1 convs have a single tap: dx, dy never move)
             cb = 0;
             if (taps9 && ++dx == 3) { dx = 0; ++dy; }
           }
           if (++stage == nstages) { stage = 0; phase ^= 1u; }
         }
-        GEMM_TRACE(leader, 1, pit);   // producer: last k-block's loads issued
       }
-      __syncwarp();
     }
-  } else if (warp == 1) {
-    // ------------------------------- MMA issuer (leader CTA only in pair mode) --
-    // The whole warp walks the loop converged (waits included) and one elected lane issues: every operand of the
-    // tcgen05 instructions is then provably warp-uniform, so they compile to bare UTCHMMA / UTCBAR with uniform-register
-    // descriptors — no per-instruction broadcast loop — and the descriptors advance by one add per operand.
-    if (rank == 0) {
-      const bool leader = elect_one();
-      const uint32_t idesc = make_idesc_f16(kPair ? 2 * kBlockM : kBlockM, p.block_n, p.is_bf16 != 0, false, false);
-      const uint32_t tmem0 = warp_uniform(tmem_base);
-      const uint32_t smem0 = warp_uniform(smem_u32(smem));
-      const uint32_t bar0 = warp_uniform(smem_u32(bars));
-      const uint32_t a_full = bar0 + static_cast<uint32_t>(offsetof(GemmBarriers, full));
-      const uint32_t a_empty = bar0 + static_cast<uint32_t>(offsetof(GemmBarriers, empty));
-      const uint32_t a_tfull = bar0 + static_cast<uint32_t>(offsetof(GemmBarriers, tmem_full));
-      const uint32_t a_tempty = bar0 + static_cast<uint32_t>(offsetof(GemmBarriers, tmem_empty));
-      const uint32_t hi = sdesc_hi_sw128(1024);
-      const uint32_t lo0 = sdesc_lo(smem0, 16);         // A of stage 0; B sits 16 KB (1024 descriptor units) behind it
-      const uint32_t lo_step = stage_bytes >> 4;
-      const int nkb = p.num_k_blocks, nstages = p.num_stages;
-      int stage = 0;
-      uint32_t phase = 0, lo = lo0;
-      int it = 0;
-      for (int item = first_item; item < num_items; item += item_step, ++it) {
-        const uint32_t acc = static_cast<uint32_t>(it) & 1u;
-        GEMM_TRACE(leader, 2, it);    // MMA: wants the accumulator
-        mbar_wait_a(a_tempty + acc * 8u, ((static_cast<uint32_t>(it) >> 1) & 1u) ^ 1u, 2);
-        tc_fence_after();
-        GEMM_TRACE(leader, 3, it);    // MMA: accumulator free
-        const uint32_t tmem_acc = tmem0 + acc * kAccStride;
-        for (int kb = 0; kb < nkb; ++kb) {
-          mbar_wait_a(a_full + static_cast<uint32_t>(stage) * 8u, phase, 3);
-          tc_fence_after();
-          GEMM_TRACE(leader && kb == 0, 4, it);   // MMA: first operands landed
-          if (leader) {
-            if constexpr (kPair) {
-#pragma unroll
-              for (int k = 0; k < kBlockK / kUmmaK; ++k) {
-                const uint64_t da = (static_cast<uint64_t>(hi) << 32) | (lo + 2u * k);
-                const uint64_t db = (static_cast<uint64_t>(hi) << 32) | (lo + 1024u + 2u * k);
-                umma_f16_ss_pair(tmem_acc, da, db, idesc, (kb | k) != 0 ? 1u : 0u);
-              }
-              umma_commit_pair(&bars->empty[stage]);  // smem slot free (in both CTAs) once these MMAs retire
-            } else {
-#pragma unroll
-              for (int k = 0; k < kBlockK / kUmmaK; ++k)
-                umma_f16_ss_lh(tmem_acc, lo + 2u * k, hi, lo + 1024u + 2u * k, hi, idesc, (kb | k) != 0 ? 1u : 0u);
-              umma_commit_a(a_empty + static_cast<uint32_t>(stage) * 8u);
-            }
-          }
-          lo += lo_step;
-          if (++stage == nstages) { stage = 0; phase ^= 1u; lo = lo0; }
-        }
-        // accumulator complete -> epilogue (of both CTAs)
-        if (leader) {
-          if constexpr (kPair) umma_commit_pair(&bars->tmem_full[acc]);
-          else umma_commit_a(a_tfull + acc * 8u);
-        }
-        GEMM_TRACE(leader, 5, it);    // MMA: last MMA issued + committed
-      }
-      __syncwarp();
-    }
-  } else {
-    // ------------------------------- epilogue warps -----------------------------
-    const int quarter = warp & 3;      // TMEM lane quarter this warp may access
-    const int group = (warp - 2) >> 2;  // warps 2-5 / 6-9: chunks group, group+2, ...
-    uint32_t uses[2] = {0u, 0u};
-    uint32_t chunk_count = 0u, d_slot = 0u;
-    int it = 0;
-    for (int item = first_item; item < num_items; item += item_step, ++it) {
-      const int acc = it & 1;
-      const uint32_t acc_phase = (it >> 1) & 1;
-      const int n_tile = item % p.num_n_tiles;
-      const int m_tile = kPair ? 2 * (item / p.num_n_tiles) + rank : item / p.num_n_tiles;
-      const uint32_t tmem_acc = tmem_base + acc * kAccStride;
-      if (p.is_bf16)
-        epilogue_tile<true>(p, &tmD, &tmR, bars, stage_d, stage_r, &bars->tmem_full[acc], acc_phase, tmem_acc, m_tile,
-                            n_tile, quarter, group, lane, uses, chunk_count, d_slot, it);
-      else
-        epilogue_tile<false>(p, &tmD, &tmR, bars, stage_d, stage_r, &bars->tmem_full[acc], acc_phase, tmem_acc, m_tile,
-                             n_tile, quarter, group, lane, uses, chunk_count, d_slot, it);
-      tc_fence_before();
-      // the MMA issuer (leader CTA) may overwrite this accumulator once BOTH CTAs have drained theirs
-      // one (possibly remote) arrival per warp: 256 remote arrivals per tile cost more than a short tile's MMAs
-      __syncwarp();
-      if (lane == 0) {
-        if constexpr (kPair) mbar_arrive_cluster(mapa_u32(smem_u32(&bars->tmem_empty[acc]), 0));
-        else mbar_arrive(&bars->tmem_empty[acc]);
-      }
-      GEMM_TRACE(lane == 0 && quarter == ((2 + 4 * group) & 3), 8 + 12 * group + 10, it);   // epilogue: accumulator released
-    }
-    bulk_wait<0>();  // the issuing threads' TMA stores must have completed before the CTA (and its smem) goes away
+    return;
   }
 
-  tc_fence_before();
-  if constexpr (kPair) cluster_sync_all();  // no CTA of the pair may exit while the other can still signal it
-  else __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    if constexpr (kPair) tmem_dealloc_pair(tmem_base, kTmemCols);
-    else tmem_dealloc(tmem_base, kTmemCols);
+  // ------------------------------- consumer warpgroups -------------------------------
+  setmaxnreg_inc<232>();
+  const int wg = warp >> 2;
+  const int row0 = wg * 64 + (warp & 3) * 16 + (lane >> 2);  // this thread's accumulator rows: row0, row0 + 8
+  const int colq = (lane & 3) * 2;                            // and columns 8g + colq, 8g + colq + 1
+  const bool signaller = (threadIdx.x & 127) == 0;            // releases stages for its warpgroup
+  const bool leader = threadIdx.x == 0;                       // issues the epilogue's TMA stores / residual loads
+  const bool geglu = (p.flags & B200SD_EPI_GEGLU) != 0;
+  const int out_bn = geglu ? BN / 2 : BN;
+  const int nchunks = out_bn / kChunkCols;
+  const uint32_t smem0 = smem_u32(smem);
+  float acc[BN / 2];
+  int stage = 0;
+  uint32_t phase = 0;
+  uint32_t res_uses[2] = {0u, 0u};
+  uint32_t d_slot = 0;
+
+  for (int item = blockIdx.x; item < num_items; item += gridDim.x) {
+    const int n_tile = item % p.num_n_tiles;
+    const int m_tile = item / p.num_n_tiles;
+    const TileCoord tc = tile_coord(p, m_tile);
+    // residual chunks 0 and 1 are fetched while the main loop runs (both buffers are free: every read of the previous
+    // tile's residual is behind the consumer barrier of its last chunk)
+    if (p.has_residual && leader) {
+      load_residual(p, &tmR, bars, stage_r, tc, n_tile, out_bn, 0);
+      if (nchunks > 1) load_residual(p, &tmR, bars, stage_r, tc, n_tile, out_bn, 1);
+    }
+
+    // main loop: one wgmma group per k-block; a stage is released once the group after it has been waited for
+    int prev_stage = 0;
+    for (int kb = 0; kb < p.num_k_blocks; ++kb) {
+      mbar_wait(&bars->full[stage], phase);
+      const uint32_t a_addr = smem0 + static_cast<uint32_t>(stage) * kStageBytes + static_cast<uint32_t>(wg) * 8192u;
+      const uint32_t b_addr = smem0 + static_cast<uint32_t>(stage) * kStageBytes + kATileBytes;
+      reg_fence(acc);
+      wgmma_fence();
+#pragma unroll
+      for (int k = 0; k < kBlockK / kMmaK; ++k)
+        Wgmma<BN, kBf16>::ss(acc, make_gdesc_sw128(a_addr + 32u * k, 16, 1024), make_gdesc_sw128(b_addr + 32u * k, 16, 1024),
+                             (kb | k) != 0 ? 1u : 0u);
+      wgmma_commit();
+      reg_fence(acc);
+      wgmma_wait<1>();
+      if (kb > 0 && signaller) mbar_arrive(&bars->empty[prev_stage]);
+      prev_stage = stage;
+      if (++stage == p.num_stages) { stage = 0; phase ^= 1u; }
+    }
+    wgmma_wait<0>();
+    reg_fence(acc);
+    if (signaller) mbar_arrive(&bars->empty[prev_stage]);
+
+    // epilogue
+    const float* bias_r[2] = {p.bias, p.bias};
+    if (p.bias != nullptr && p.bias_group_rows > 0) {
+#pragma unroll
+      for (int h = 0; h < 2; ++h) bias_r[h] = p.bias + (tile_row(p, tc, m_tile, row0 + 8 * h) / p.bias_group_rows) * p.N;
+    }
+#pragma unroll
+    for (int c = 0; c < BN / kChunkCols; ++c) {
+      if (c < nchunks) {
+        float f[2][4][2];  // [row half][8-column group][column]
+#pragma unroll
+        for (int g = 0; g < 4; ++g) {
+          const int col = n_tile * BN + c * kChunkCols + g * 8 + colq;  // column in the [N] space of the GEMM
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {
+            float2 b = make_float2(0.f, 0.f), bg = make_float2(0.f, 0.f);
+            if (p.bias != nullptr) {
+              b = __ldg(reinterpret_cast<const float2*>(bias_r[h] + col));
+              if (geglu) bg = __ldg(reinterpret_cast<const float2*>(bias_r[h] + col + BN / 2));
+            }
+#pragma unroll
+            for (int e = 0; e < 2; ++e) {
+              const int idx = 4 * (4 * c + g) + 2 * h + e;
+              float v = acc[idx] + (e ? b.y : b.x);
+              if (geglu) {
+                constexpr int kGate = BN / 4;  // accumulator index distance of column + BN/2
+                v *= gelu_erf(acc[(idx + kGate) % (BN / 2)] + (e ? bg.y : bg.x));
+              }
+              f[h][g][e] = v;
+            }
+          }
+        }
+        if (p.has_residual) {
+          const int buf = c & 1;
+          mbar_wait(&bars->res_full[buf], res_uses[buf] & 1u);
+          res_uses[buf]++;
+          const uint8_t* rt = stage_r + buf * kStageTileBytes;
+#pragma unroll
+          for (int h = 0; h < 2; ++h)
+#pragma unroll
+            for (int g = 0; g < 4; ++g) {
+              const float2 t = unpack2<kBf16>(*reinterpret_cast<const uint32_t*>(rt + sw64_offset(row0 + 8 * h, g) + colq * 2));
+              f[h][g][0] += t.x;
+              f[h][g][1] += t.y;
+            }
+        }
+        if (p.flags & B200SD_EPI_SILU) {
+#pragma unroll
+          for (int h = 0; h < 2; ++h)
+#pragma unroll
+            for (int g = 0; g < 4; ++g)
+#pragma unroll
+              for (int e = 0; e < 2; ++e) f[h][g][e] = __fdividef(f[h][g][e], 1.0f + __expf(-f[h][g][e]));
+        }
+        uint8_t* dt = stage_d + d_slot * kStageTileBytes;
+#pragma unroll
+        for (int h = 0; h < 2; ++h)
+#pragma unroll
+          for (int g = 0; g < 4; ++g)
+            *reinterpret_cast<uint32_t*>(dt + sw64_offset(row0 + 8 * h, g) + colq * 2) = pack2<kBf16>(f[h][g][0], f[h][g][1]);
+        fence_proxy_async_smem();  // my staging writes (and residual reads) -> visible / ordered for the async proxy
+        // the buffer the next chunk is staged into was last read by the previous store: it must be done reading
+        if (leader) bulk_wait_read<0>();
+        consumer_bar_sync();
+        if (leader) {
+          const int col = n_tile * out_bn + c * kChunkCols;
+          if (p.mode == 0) tma_store_2d(&tmD, dt, col, tc.c1);
+          else tma_store_4d(&tmD, dt, col, tc.c1, tc.c2, tc.c3);
+          bulk_commit();
+          if (p.has_residual && c + 2 < nchunks) load_residual(p, &tmR, bars, stage_r, tc, n_tile, out_bn, c + 2);
+        }
+        d_slot ^= 1u;
+      }
+    }
   }
+  if (leader) bulk_wait<0>();  // the TMA stores must have completed before the CTA (and its smem) goes away
 }
 
 // ------------------------------------------------------------------------------------------------
 // host side
 // ------------------------------------------------------------------------------------------------
-static long long* g_gemm_trace = nullptr;
+typedef void (*GemmKernel)(CUtensorMap, CUtensorMap, CUtensorMap, CUtensorMap, GemmKernelParams);
+
+template <bool kBf16>
+static GemmKernel kernel_for(int block_n) {
+  switch (block_n) {
+    case 32: return gemm_conv_tc_kernel<32, kBf16>;
+    case 64: return gemm_conv_tc_kernel<64, kBf16>;
+    case 96: return gemm_conv_tc_kernel<96, kBf16>;
+    case 128: return gemm_conv_tc_kernel<128, kBf16>;
+    case 160: return gemm_conv_tc_kernel<160, kBf16>;
+    case 192: return gemm_conv_tc_kernel<192, kBf16>;
+    case 224: return gemm_conv_tc_kernel<224, kBf16>;
+    case 256: return gemm_conv_tc_kernel<256, kBf16>;
+    default: return nullptr;
+  }
+}
+static GemmKernel kernel_for(int block_n, int is_bf16) {
+  return is_bf16 ? kernel_for<true>(block_n) : kernel_for<false>(block_n);
+}
+
 static int g_num_sms = 0;
 static int g_max_smem = 0;
 static bool g_dev_ready[64] = {};
@@ -710,10 +395,10 @@ static int device_props() {
     if (cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess) return B200SD_ERR_CUDA;
     if (cudaDeviceGetAttribute(&smem, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev) != cudaSuccess)
       return B200SD_ERR_CUDA;
-    if (cudaFuncSetAttribute(gemm_conv_tc_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem) !=
-            cudaSuccess ||
-        cudaFuncSetAttribute(gemm_conv_tc_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem) != cudaSuccess)
-      return B200SD_ERR_CUDA;
+    for (int bn = 32; bn <= 256; bn += 32)
+      for (int bf = 0; bf < 2; ++bf)
+        if (cudaFuncSetAttribute(kernel_for(bn, bf), cudaFuncAttributeMaxDynamicSharedMemorySize, smem) != cudaSuccess)
+          return B200SD_ERR_CUDA;
     g_num_sms = sms;
     g_max_smem = smem;
     g_dev_ready[dev] = true;
@@ -721,92 +406,24 @@ static int device_props() {
   return B200SD_OK;
 }
 
-// Pair mode pays when it shortens the (waves x per-tile time) product: a pair tile does two M tiles in the time of
-// one, and its per-SM smem fill per FLOP is lower (B is split between the two CTAs), so the L2->SM port (~64 B/clk/SM,
-// the limiter of 128-row tiles: ncu round 1) caps the tensor pipe later.  eff = min(1, arithmetic intensity / 128).
-static int pair_env() {
-  static int v = -2;
-  if (v == -2) {
-    const char* e = getenv("B200SD_PAIR");
-    // 0 = never (default), 1 = whenever legal, -1 = the cost model below.  Round-1 measurement (bench.py, batch 32):
-    // pair mode is correct (tests/test_kernels_gpu.py under B200SD_PAIR=1) but 1-3 % slower than 128-row tiles on
-    // this UNet's shapes, so it stays opt-in until the cause is profiled.
-    v = e ? atoi(e) : 0;
-  }
-  return v;
-}
-static bool decide_pair(const GemmKernelParams& p, int num_sms) {
-  if (p.num_m_tiles < 2 || p.block_n % 32 != 0 || p.block_n < 64) return false;
-  const int env = pair_env();
-  if (env == 0) return false;
-  if (env == 1) return true;
-  const double bn = p.block_n;
-  const double eff1 = fmin(1.0, bn / (128.0 + bn));
-  const double eff2 = fmin(1.0, bn / (128.0 + 0.5 * bn));
-  const long long items1 = static_cast<long long>(p.num_m_tiles) * p.num_n_tiles;
-  const long long items2 = static_cast<long long>((p.num_m_tiles + 1) / 2) * p.num_n_tiles;
-  const double t1 = static_cast<double>((items1 + num_sms - 1) / num_sms) / eff1;
-  const double t2 = static_cast<double>((items2 + num_sms / 2 - 1) / (num_sms / 2)) / eff2;
-  return t2 < 0.97 * t1;
-}
-
 static int launch(const CUtensorMap& tmA, const CUtensorMap& tmB, const CUtensorMap& tmD, const CUtensorMap& tmR,
-                  GemmKernelParams& p, int max_ctas, cudaStream_t stream) {
-  const int bn_local = p.pair ? p.block_n / 2 : p.block_n;
-  const uint32_t stage_bytes = 16384u + static_cast<uint32_t>(bn_local) * 128u;
-  // Output staging: a third buffer per epilogue group lets the TMA store of chunk i-1 keep reading while chunk i is
-  // staged (with two, every chunk waits for the previous store's shared-memory read).  Measured (tools/gemm_sweep.py,
-  // K = 320 / 1280 linears): no gain — those GEMMs sit at 70-85 % of their HBM roofline, not on the store latency — so
-  // two buffers stay the default and B200SD_GEMM_DBUFS=3 remains an experiment knob.
-  static int dbufs_env = -1;
-  if (dbufs_env < 0) {
-    const char* e = getenv("B200SD_GEMM_DBUFS");
-    dbufs_env = e ? atoi(e) : 0;
-  }
-  p.d_bufs = dbufs_env == 3 ? 3 : 2;
-  p.trace = g_gemm_trace;
-  const int staging = p.d_bufs * 2 * static_cast<int>(kStageTileBytes) + (p.has_residual ? static_cast<int>(kStagingBytes) : 0);
-  const int budget = g_max_smem - 1024 /*align*/ - staging - static_cast<int>(sizeof(GemmBarriers)) - 64;
+                  GemmKernelParams& p, int is_bf16, int max_ctas, cudaStream_t stream) {
+  const uint32_t stage_bytes = kATileBytes + static_cast<uint32_t>(p.block_n) * 128u;
+  const int staging = (p.has_residual ? 4 : 2) * static_cast<int>(kStageTileBytes);
+  const int budget = g_max_smem - 1024 /*align*/ - staging - static_cast<int>(sizeof(GemmBarriers));
   int stages = budget / static_cast<int>(stage_bytes);
   if (stages > kMaxStages) stages = kMaxStages;
-  {
-    static int cap = -1;  // experiment knob: B200SD_GEMM_STAGES caps the operand ring depth
-    if (cap < 0) {
-      const char* e = getenv("B200SD_GEMM_STAGES");
-      cap = e ? atoi(e) : 0;
-    }
-    if (cap >= 2 && stages > cap) stages = cap;
-  }
   if (stages < 2) return B200SD_ERR_UNSUPPORTED;
   p.num_stages = stages;
-  size_t smem = 1024 + static_cast<size_t>(stages) * stage_bytes + staging + sizeof(GemmBarriers) + 64;
-  if (smem < 120 * 1024) smem = 120 * 1024;  // one CTA per SM: the kernel owns all 512 TMEM columns
-  if (!p.pair) {
-    const int num_tiles = p.num_m_tiles * p.num_n_tiles;
-    int grid = num_tiles < g_num_sms ? num_tiles : g_num_sms;
-    if (max_ctas > 0 && grid > max_ctas) grid = max_ctas;
-    if (grid <= 0) return B200SD_OK;
-    launch_pdl(gemm_conv_tc_kernel<false>, dim3(grid), dim3(kGemmThreads), smem, stream, tmA, tmB, tmD, tmR, p);
-    return cudaGetLastError() == cudaSuccess ? B200SD_OK : B200SD_ERR_CUDA;
-  }
-  const int num_items = ((p.num_m_tiles + 1) / 2) * p.num_n_tiles;
-  int clusters = num_items < g_num_sms / 2 ? num_items : g_num_sms / 2;
-  if (max_ctas > 1 && clusters > max_ctas / 2) clusters = max_ctas / 2;
-  if (clusters <= 0) return B200SD_OK;
-  cudaLaunchConfig_t cfg{};
-  cfg.gridDim = dim3(2 * clusters);
-  cfg.blockDim = dim3(kGemmThreads);
-  cfg.dynamicSmemBytes = smem;
-  cfg.stream = stream;
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeClusterDimension;
-  attr[0].val.clusterDim.x = 2;
-  attr[0].val.clusterDim.y = 1;
-  attr[0].val.clusterDim.z = 1;
-  cfg.attrs = attr;
-  cfg.numAttrs = 1;
-  return cudaLaunchKernelEx(&cfg, gemm_conv_tc_kernel<true>, tmA, tmB, tmD, tmR, p) == cudaSuccess ? B200SD_OK
-                                                                                                    : B200SD_ERR_CUDA;
+  const size_t smem = 1024 + static_cast<size_t>(stages) * stage_bytes + staging + sizeof(GemmBarriers);
+  const int num_tiles = p.num_m_tiles * p.num_n_tiles;
+  int grid = num_tiles < g_num_sms ? num_tiles : g_num_sms;
+  if (max_ctas > 0 && grid > max_ctas) grid = max_ctas;
+  if (grid <= 0) return B200SD_OK;
+  GemmKernel k = kernel_for(p.block_n, is_bf16);
+  if (k == nullptr) return B200SD_ERR_INVALID;
+  launch_pdl(k, dim3(grid), dim3(kGemmThreads), smem, stream, tmA, tmB, tmD, tmR, p);
+  return cudaGetLastError() == cudaSuccess ? B200SD_OK : B200SD_ERR_CUDA;
 }
 
 struct OutSpec {
@@ -827,7 +444,6 @@ static int fill_common(GemmKernelParams& p, OutSpec& o, int M, int N, int K, int
   p.bias = epi ? epi->bias : nullptr;
   p.bias_group_rows = epi ? epi->bias_group_rows : 0;
   p.flags = epi ? epi->flags : 0;
-  p.is_bf16 = is_bf16;
   o.D = D; o.ldd = ldd;
   o.residual = epi ? epi->residual : nullptr;
   o.ldr = epi ? epi->ldr : 0;
@@ -888,8 +504,6 @@ int gemm_tc(const void* A, long long lda, const void* Wt, void* D, long long ldd
   p.d_bytes = kStageTileBytes;
   rc = device_props();
   if (rc != B200SD_OK) return rc;
-  p.pair = decide_pair(p, g_num_sms) ? 1 : 0;
-  if (p.pair) p.b_bytes /= 2;
   CUtensorMap tmA, tmB, tmD, tmR;
   {
     const uint64_t dims[2] = {static_cast<uint64_t>(K), static_cast<uint64_t>(M)};
@@ -902,14 +516,14 @@ int gemm_tc(const void* A, long long lda, const void* Wt, void* D, long long ldd
   {
     const uint64_t dims[2] = {static_cast<uint64_t>(K), static_cast<uint64_t>(N)};
     const uint64_t strides[1] = {static_cast<uint64_t>(K) * 2};
-    const uint32_t box[2] = {kBlockK, static_cast<uint32_t>(p.pair ? block_n / 2 : block_n)};
+    const uint32_t box[2] = {kBlockK, static_cast<uint32_t>(block_n)};
     const uint32_t es[2] = {1, 1};
     rc = make_tmap_sw128(&tmB, Wt, 2, dims, strides, box, es);
     if (rc != B200SD_OK) return rc;
   }
   rc = make_out_maps(p, o, &tmD, &tmR);
   if (rc != B200SD_OK) return rc;
-  return launch(tmA, tmB, tmD, tmR, p, max_ctas, stream);
+  return launch(tmA, tmB, tmD, tmR, p, is_bf16, max_ctas, stream);
 }
 
 int conv_tc(const void* X, long long pitch_c, int NB, int Hin, int Win, int C, const void* Wt, int ksize, int stride,
@@ -943,8 +557,6 @@ int conv_tc(const void* X, long long pitch_c, int NB, int Hin, int Win, int C, c
   p.d_bytes = static_cast<uint32_t>(p.bw * p.bh * p.bn) * kChunkCols * 2u;
   rc = device_props();
   if (rc != B200SD_OK) return rc;
-  p.pair = decide_pair(p, g_num_sms) ? 1 : 0;
-  if (p.pair) p.b_bytes /= 2;
   CUtensorMap tmA, tmB, tmD, tmR;
   {
     const uint64_t dims[4] = {static_cast<uint64_t>(C), static_cast<uint64_t>(Win), static_cast<uint64_t>(Hin),
@@ -963,21 +575,20 @@ int conv_tc(const void* X, long long pitch_c, int NB, int Hin, int Win, int C, c
     const uint64_t K = static_cast<uint64_t>(taps) * C;
     const uint64_t dims[2] = {K, static_cast<uint64_t>(Cout)};
     const uint64_t strides[1] = {K * 2};
-    const uint32_t box[2] = {kBlockK, static_cast<uint32_t>(p.pair ? block_n / 2 : block_n)};
+    const uint32_t box[2] = {kBlockK, static_cast<uint32_t>(block_n)};
     const uint32_t es[2] = {1, 1};
     rc = make_tmap_sw128(&tmB, Wt, 2, dims, strides, box, es);
     if (rc != B200SD_OK) return rc;
   }
   rc = make_out_maps(p, o, &tmD, &tmR);
   if (rc != B200SD_OK) return rc;
-  return launch(tmA, tmB, tmD, tmR, p, max_ctas, stream);
+  return launch(tmA, tmB, tmD, tmR, p, is_bf16, max_ctas, stream);
 }
 
 }  // namespace b200sd
 
-// debug hook: device buffer of 32 * 64 int64 that CTA 0 of later GEMM / conv launches fills with clock64 stamps (only in
-// builds with -DB200SD_GEMM_TRACE_ENABLE=1; tools/gemm_trace.py)
+// debug hook kept for ABI compatibility: the sm_90a GEMM / conv kernel records no timeline, so the buffer is never written
 extern "C" int b200sd_debug_gemm_trace(void* device_buffer) {
-  b200sd::g_gemm_trace = static_cast<long long*>(device_buffer);
+  (void)device_buffer;
   return B200SD_OK;
 }

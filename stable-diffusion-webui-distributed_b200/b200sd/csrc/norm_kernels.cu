@@ -51,27 +51,17 @@ __device__ __forceinline__ uint4 pack8(const float (&f)[8]) {
   return make_uint4(w[0], w[1], w[2], w[3]);
 }
 
-// Blackwell packed fp32 (two lanes per instruction: FADD2 / FMUL2 / FFMA2) — these kernels are instruction-issue bound
-// before they are HBM bound when every element costs a scalar convert + add + fma.
-struct F2 { uint64_t v; };
-__device__ __forceinline__ F2 f2_make(float x, float y) {
-  F2 r;
-  asm("mov.b64 %0, {%1, %2};" : "=l"(r.v) : "r"(__float_as_uint(x)), "r"(__float_as_uint(y)));
-  return r;
-}
+// Pairs of fp32 lanes.  sm_90 has no packed fp32 pipe, so each pair op is two scalar round-to-nearest ops — the
+// same per-lane results the packed form gives.
+struct F2 { float x, y; };
+__device__ __forceinline__ F2 f2_make(float x, float y) { return F2{x, y}; }
 __device__ __forceinline__ void f2_get(F2 a, float& x, float& y) {
-  uint32_t lo, hi;
-  asm("mov.b64 {%0, %1}, %2;" : "=r"(lo), "=r"(hi) : "l"(a.v));
-  x = __uint_as_float(lo);
-  y = __uint_as_float(hi);
+  x = a.x;
+  y = a.y;
 }
-__device__ __forceinline__ F2 f2_add(F2 a, F2 b) { F2 r; asm("add.rn.f32x2 %0, %1, %2;" : "=l"(r.v) : "l"(a.v), "l"(b.v)); return r; }
-__device__ __forceinline__ F2 f2_mul(F2 a, F2 b) { F2 r; asm("mul.rn.f32x2 %0, %1, %2;" : "=l"(r.v) : "l"(a.v), "l"(b.v)); return r; }
-__device__ __forceinline__ F2 f2_fma(F2 a, F2 b, F2 c) {
-  F2 r;
-  asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(r.v) : "l"(a.v), "l"(b.v), "l"(c.v));
-  return r;
-}
+__device__ __forceinline__ F2 f2_add(F2 a, F2 b) { return F2{__fadd_rn(a.x, b.x), __fadd_rn(a.y, b.y)}; }
+__device__ __forceinline__ F2 f2_mul(F2 a, F2 b) { return F2{__fmul_rn(a.x, b.x), __fmul_rn(a.y, b.y)}; }
+__device__ __forceinline__ F2 f2_fma(F2 a, F2 b, F2 c) { return F2{__fmaf_rn(a.x, b.x, c.x), __fmaf_rn(a.y, b.y, c.y)}; }
 template <bool kBf16>
 __device__ __forceinline__ void unpack4x2(const uint4& u, F2 (&f)[4]) {
   const uint32_t w[4] = {u.x, u.y, u.z, u.w};
@@ -579,8 +569,8 @@ layernorm_kernel(const uint8_t* __restrict__ X, long long ldx, uint8_t* __restri
 // with 1-D bulk copies (cp.async.bulk: the TMA engine without a tensor map), the normalised rows leave through two
 // private output stages by bulk stores, and nothing but __syncwarp and the warp's own mbarriers synchronises — a first
 // version with one producer warp and CTA-wide barriers per 20 KB tile spent 2.3 us per tile in hand-offs (2.6 TB/s with
-// one CTA per SM whatever the ring depth).  The arithmetic is packed fp32 (FADD2 / FFMA2, two accumulators): with a
-// scalar convert + add + fma per element the kernel was instruction-issue bound at 4.3 TB/s.
+// one CTA per SM whatever the ring depth).  The arithmetic runs on pairs of
+// values with two accumulators (F2 above; two scalar ops per pair on sm_90).
 constexpr int kLnWarps = 16;
 constexpr int kLnThreads = 32 * kLnWarps;
 constexpr int kLnInDefault = 3, kLnOutDefault = 2;  // input / output stages per warp (B200SD_LN_STAGES="in,out")
@@ -648,7 +638,7 @@ layernorm_staged_kernel(const uint8_t* __restrict__ X, long long ldx, uint8_t* _
   for (int tile = tile0; tile < num_tiles; tile += tile_step) {
     const int r0 = tile * rpw, nr = min(rpw, rows - r0);
     const bool live = wrow < nr;      // whole-warp shuffles below: dead rows just carry zeros
-    mbar_wait(&full[s], par, 32);
+    mbar_wait(&full[s], par);
     const uint8_t* xr = in_st + s * tile_bytes + static_cast<uint32_t>(wrow) * row_bytes;
     F2 f[VPT][4];                      // my 8 * VPT elements as fp32 pairs
     F2 acc0 = f2_make(0.f, 0.f), acc1 = acc0;
@@ -697,11 +687,12 @@ layernorm_staged_kernel(const uint8_t* __restrict__ X, long long ldx, uint8_t* _
     for (int it = 0; it < VPT; ++it) {
       const int vec = it * lpr + sub;
       if (live && vec < nvec) {
-        const ulonglong2 g0 = *reinterpret_cast<const ulonglong2*>(gb + vec * 8);
-        const ulonglong2 g1 = *reinterpret_cast<const ulonglong2*>(gb + vec * 8 + 4);
-        const ulonglong2 b0 = *reinterpret_cast<const ulonglong2*>(gb + C + vec * 8);
-        const ulonglong2 b1 = *reinterpret_cast<const ulonglong2*>(gb + C + vec * 8 + 4);
-        const F2 gg[4] = {{g0.x}, {g0.y}, {g1.x}, {g1.y}}, bb[4] = {{b0.x}, {b0.y}, {b1.x}, {b1.y}};
+        const float4 g0 = *reinterpret_cast<const float4*>(gb + vec * 8);
+        const float4 g1 = *reinterpret_cast<const float4*>(gb + vec * 8 + 4);
+        const float4 b0 = *reinterpret_cast<const float4*>(gb + C + vec * 8);
+        const float4 b1 = *reinterpret_cast<const float4*>(gb + C + vec * 8 + 4);
+        const F2 gg[4] = {{g0.x, g0.y}, {g0.z, g0.w}, {g1.x, g1.y}, {g1.z, g1.w}};
+        const F2 bb[4] = {{b0.x, b0.y}, {b0.z, b0.w}, {b1.x, b1.y}, {b1.z, b1.w}};
         uint32_t w[4];
 #pragma unroll
         for (int i = 0; i < 4; ++i) w[i] = pack2<kBf16>(f2_fma(f2_mul(f[it][i], rstd2), gg[i], bb[i]));
@@ -1042,7 +1033,7 @@ extern "C" int b200sd_layernorm(const void* X, long long ldx, void* Y, long long
     blocks = (rows + (32 / lpr) * kLnWarps - 1) / ((32 / lpr) * kLnWarps);
     int per_sm = sh_staged + 1024 <= 113 * 1024 ? 2 : 1;
     if (ctas_per_sm > 0) per_sm = ctas_per_sm;
-    if (blocks > 148 * per_sm) blocks = 148 * per_sm;
+    if (blocks > kNumSms * per_sm) blocks = kNumSms * per_sm;
     if (dtype == B200SD_BF16)
       launch_ln_staged<true>(n_in, n_out, vpt, lpr, blocks, sh_staged, st, static_cast<const uint8_t*>(X), ldx,
                              static_cast<uint8_t*>(Y), ldy, rows, C, gamma, beta, eps);
@@ -1051,7 +1042,7 @@ extern "C" int b200sd_layernorm(const void* X, long long ldx, void* Y, long long
                               static_cast<uint8_t*>(Y), ldy, rows, C, gamma, beta, eps);
     return cudaGetLastError() == cudaSuccess ? B200SD_OK : B200SD_ERR_CUDA;
   }
-  if (blocks > 148 * 8) blocks = 148 * 8;
+  if (blocks > kNumSms * 8) blocks = kNumSms * 8;
   const size_t sh = 2 * static_cast<size_t>(C) * sizeof(float);
   if (dtype == B200SD_BF16)
     launch_ln<true>(vpt, lpr, blocks, sh, st, static_cast<const uint8_t*>(X), ldx, static_cast<uint8_t*>(Y), ldy, rows, C,

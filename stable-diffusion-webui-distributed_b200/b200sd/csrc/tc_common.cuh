@@ -1,6 +1,6 @@
-// tc_common.cuh — sm_100a building blocks shared by the tensor-core kernels:
-// mbarrier, TMA (cp.async.bulk.tensor), tcgen05 (alloc / mma / commit / ld / st) wrappers,
-// UMMA shared-memory and instruction descriptors.  Inline PTX only; no CUTLASS dependency.
+// tc_common.cuh — sm_90a building blocks shared by the tensor-core kernels:
+// mbarrier, TMA (cp.async.bulk.tensor), wgmma fences and shared-memory descriptors.
+// Inline PTX only; no CUTLASS dependency.
 #pragma once
 #include <cuda.h>
 #include <cuda_bf16.h>
@@ -22,18 +22,6 @@ __device__ __forceinline__ float fast_exp2(float x) {
   return y;
 }
 
-__device__ __forceinline__ bool elect_one() {
-  uint32_t pred = 0;
-  asm volatile(
-      "{\n\t"
-      ".reg .pred P;\n\t"
-      "elect.sync _|P, 0xffffffff;\n\t"
-      "selp.b32 %0, 1, 0, P;\n\t"
-      "}\n"
-      : "=r"(pred));
-  return pred != 0;
-}
-
 // ----------------------------------------------------------------------------------------------
 // mbarrier
 // ----------------------------------------------------------------------------------------------
@@ -50,16 +38,14 @@ __device__ __forceinline__ void mbar_arrive_expect_tx(uint64_t* bar, uint32_t by
 __device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
   asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
 }
-// B200SD_WAIT_HINT_NS > 0: every mbar_wait carries a suspend-time hint (the waiting thread sleeps in hardware and is
-// woken by barrier traffic) instead of re-issuing the poll back to back.  Measured on B200 (tools/gemm_sweep.py,
-// tools/attn_sweep.py): without the hint the polling warps take issue slots from the MMA-issuing thread and the
-// epilogue / softmax warps — 3x3 conv 980 -> 1082 TFLOP/s, attention 1.00 -> 0.91 ms; 500 ns and 20 us behave the same.
+// Every wait carries a suspend-time hint (B200SD_WAIT_HINT_NS): the waiting thread sleeps in hardware and is woken by
+// barrier traffic instead of re-issuing the poll back to back, so waiting warps leave their issue slots to the warps
+// doing the math.
 #ifndef B200SD_WAIT_HINT_NS
 #define B200SD_WAIT_HINT_NS 20000
 #endif
 __device__ __forceinline__ bool mbar_try_wait(uint64_t* bar, uint32_t parity) {
   uint32_t ok;
-#if B200SD_WAIT_HINT_NS > 0
   asm volatile(
       "{\n\t"
       ".reg .pred P;\n\t"
@@ -69,58 +55,17 @@ __device__ __forceinline__ bool mbar_try_wait(uint64_t* bar, uint32_t parity) {
       : "=r"(ok)
       : "r"(smem_u32(bar)), "r"(parity), "r"(static_cast<uint32_t>(B200SD_WAIT_HINT_NS))
       : "memory");
-#else
-  asm volatile(
-      "{\n\t"
-      ".reg .pred P;\n\t"
-      "mbarrier.try_wait.parity.shared::cta.b64 P, [%1], %2;\n\t"
-      "selp.b32 %0, 1, 0, P;\n\t"
-      "}\n"
-      : "=r"(ok)
-      : "r"(smem_u32(bar)), "r"(parity)
-      : "memory");
-#endif
   return ok != 0;
 }
-// Bounded wait: a protocol bug traps (CUDA error on the host) instead of hanging the GPU box.
+// Bounded wait: a protocol bug traps (CUDA error on the host) instead of hanging the GPU.  No printf here: a call in
+// the kernel would make ptxas serialise the wgmma pipeline and spill the accumulators around it.
 #ifndef B200SD_SPIN_LIMIT
-#define B200SD_SPIN_LIMIT (1u << 26)
+#define B200SD_SPIN_LIMIT (1u << 22)
 #endif
-__device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity, int tag = 0) {
+__device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
   uint32_t spins = 0;
   while (!mbar_try_wait(bar, parity)) {
-    if (++spins > (B200SD_WAIT_HINT_NS > 0 ? (B200SD_SPIN_LIMIT >> 4) : B200SD_SPIN_LIMIT)) {  // hinted polls sleep
-      printf("b200sd: mbarrier timeout tag=%d block=(%d,%d,%d) thread=%d parity=%u\n", tag, blockIdx.x, blockIdx.y,
-             blockIdx.z, threadIdx.x, parity);
-      __trap();
-    }
-  }
-}
-
-// Shared-space-address variants for hot loops: no generic->shared conversion per call, and the try_wait carries a
-// suspend-time hint so a waiting warp sleeps in hardware instead of re-issuing the poll (which would compete for issue
-// slots with the warps that do the math).
-__device__ __forceinline__ void mbar_arrive_a(uint32_t bar) {
-  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory");
-}
-__device__ __forceinline__ void mbar_wait_a(uint32_t bar, uint32_t parity, int tag = 0) {
-  uint32_t spins = 0, ok;
-  for (;;) {
-    asm volatile(
-        "{\n\t"
-        ".reg .pred P;\n\t"
-        "mbarrier.try_wait.parity.shared::cta.b64 P, [%1], %2, %3;\n\t"
-        "selp.b32 %0, 1, 0, P;\n\t"
-        "}\n"
-        : "=r"(ok)
-        : "r"(bar), "r"(parity), "r"(20000u)
-        : "memory");
-    if (ok) break;
-    if (++spins > (B200SD_SPIN_LIMIT >> 4)) {
-      printf("b200sd: mbarrier timeout tag=%d block=(%d,%d,%d) thread=%d parity=%u\n", tag, blockIdx.x, blockIdx.y,
-             blockIdx.z, threadIdx.x, parity);
-      __trap();
-    }
+    if (++spins > B200SD_SPIN_LIMIT) __trap();
   }
 }
 
@@ -155,236 +100,52 @@ __device__ __forceinline__ void tma_load_4d(void* dst, const CUtensorMap* m, uin
 __device__ __forceinline__ void fence_proxy_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 
 // ----------------------------------------------------------------------------------------------
-// tcgen05: TMEM allocation
+// wgmma (sm_90a warpgroup MMA): the four warps of a warpgroup issue together; operands are read from shared memory
+// through descriptors (or A from registers), the fp32 accumulator lives in the warpgroup's registers.
 // ----------------------------------------------------------------------------------------------
-__device__ __forceinline__ void tmem_alloc(uint32_t* dst_smem, uint32_t ncols) {  // whole warp, ncols pow2 >= 32
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(dst_smem)),
-               "r"(ncols)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
+// registers / shared memory written before this point are visible to the wgmma instructions issued after it
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+// all but the newest N committed wgmma groups of this warpgroup have completed
+template <int N>
+__device__ __forceinline__ void wgmma_wait() {
+  asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory");
 }
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {  // whole warp (the allocating one)
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
+// per-thread register budget of the executing warpgroup, changed at run time (warp-specialised kernels hand the producer's
+// registers to the math warpgroups); every warp of the warpgroup executes it
+template <int N>
+__device__ __forceinline__ void setmaxnreg_inc() {
+  asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(N) : "memory");
 }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-
-// ----------------------------------------------------------------------------------------------
-// tcgen05.mma (kind::f16: fp16/bf16 operands from shared memory, fp32 accumulate in TMEM)
-//   D[tmem] (+)= A[smem] * B[smem]^T      (A: M x K, B: N x K in the "K-major" convention)
-// Issued by ONE thread.
-// ----------------------------------------------------------------------------------------------
-__device__ __forceinline__ void umma_f16_ss(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc,
-                                            uint32_t accumulate) {
-  asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t"
-      "}\n" ::"r"(tmem_d),
-      "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
+template <int N>
+__device__ __forceinline__ void setmaxnreg_dec() {
+  asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N) : "memory");
 }
-// Arrive on an mbarrier when all previously issued tcgen05.mma of this thread have completed.
-// (implies tcgen05.fence::before_thread_sync)
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar))
-               : "memory");
+// Keeps the compiler from moving reads / writes of an accumulator across a wgmma fence, commit or wait.
+template <int N>
+__device__ __forceinline__ void reg_fence(float (&d)[N]) {
+#pragma unroll
+  for (int i = 0; i < N; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
 
-// Instruction descriptor, kind::f16 (cute::UMMA::InstrDescriptor bit layout):
-//  [4,6) c_format (1 = F32)  [7,10) a_format (0 = F16, 1 = BF16)  [10,13) b_format
-//  [15] a_major (0 = K-major, 1 = MN-major)  [16] b_major  [17,23) N>>3  [24,29) M>>4
-__host__ __device__ constexpr uint32_t make_idesc_f16(int M, int N, bool bf16, bool a_mn_major, bool b_mn_major) {
-  return (1u << 4) | ((bf16 ? 1u : 0u) << 7) | ((bf16 ? 1u : 0u) << 10) | ((a_mn_major ? 1u : 0u) << 15) |
-         ((b_mn_major ? 1u : 0u) << 16) | (static_cast<uint32_t>(N >> 3) << 17) |
-         (static_cast<uint32_t>(M >> 4) << 24);
-}
-
-// Shared-memory matrix descriptor (cute::UMMA::SmemDescriptor bit layout), SWIZZLE_128B:
-//  [0,14) start>>4  [16,30) LBO>>4  [32,46) SBO>>4  [46,48) version = 1  [61,64) layout = 2 (SW128)
+// Shared-memory matrix descriptor (wgmma), SWIZZLE_128B:
+//  [0,14) start>>4  [16,30) LBO>>4  [32,46) SBO>>4  [62,64) layout (1 = SWIZZLE_128B)
 // K-major tile (rows x 64 halfs, 128 B per row, TMA SWIZZLE_128B): SBO = 1024 B (8-row group), LBO unused (1).
+// Advancing K by 16 elements inside the 128-byte row adds 32 B to the start address.
 // MN-major tile (k-rows x 64 halfs of MN): SBO = 1024 B (8 k-rows), LBO = byte distance between 64-wide MN chunks.
-__device__ __forceinline__ uint64_t make_sdesc_sw128(uint32_t smem_addr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
+__device__ __forceinline__ uint64_t make_gdesc_sw128(uint32_t smem_addr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
   uint64_t d = 0;
   d |= static_cast<uint64_t>((smem_addr & 0x3FFFF) >> 4);
   d |= static_cast<uint64_t>((lbo_bytes >> 4) & 0x3FFF) << 16;
   d |= static_cast<uint64_t>((sbo_bytes >> 4) & 0x3FFF) << 32;
-  d |= static_cast<uint64_t>(1) << 46;
-  d |= static_cast<uint64_t>(2) << 61;
+  d |= static_cast<uint64_t>(1) << 62;
   return d;
 }
-
-// Lean forms for the MMA-issue loops.  One thread issues every tcgen05.mma of a CTA, and under contention with the
-// math warps of its SM sub-partition it retires roughly one instruction per 7 clocks, so every instruction in that loop
-// is on the kernel's critical path (measured with tools/attn_trace.py: ~160 clocks per issued MMA before this).
-// The 64-bit descriptor is (lo, hi): lo = addr>>4 | (LBO>>4)<<16 advances by plain adds (shared addresses stay below
-// 2^18, no carry into the LBO field), hi = SBO>>4 | version 1 (bit 14) | SWIZZLE_128B (2 << 29) is a constant.
-__device__ __forceinline__ uint32_t sdesc_lo(uint32_t smem_addr, uint32_t lbo_bytes) {
-  return ((smem_addr & 0x3FFFFu) >> 4) | (((lbo_bytes >> 4) & 0x3FFFu) << 16);
-}
-__device__ __forceinline__ uint32_t sdesc_hi_sw128(uint32_t sbo_bytes) {
-  return ((sbo_bytes >> 4) & 0x3FFFu) | (1u << 14) | (2u << 29);
-}
-__device__ __forceinline__ void umma_f16_ss_lh(uint32_t tmem_d, uint32_t a_lo, uint32_t a_hi, uint32_t b_lo, uint32_t b_hi,
-                                               uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      ".reg .b64 da, db;\n\t"
-      "setp.ne.b32 p, %6, 0;\n\t"
-      "mov.b64 da, {%1, %2};\n\t"
-      "mov.b64 db, {%3, %4};\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], da, db, %5, p;\n\t"
-      "}\n" ::"r"(tmem_d),
-      "r"(a_lo), "r"(a_hi), "r"(b_lo), "r"(b_hi), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// same with the A operand in TMEM (lane = row, 32-bit column j = K elements 2j, 2j+1): the P.V product of the attention
-// kernel when P is written back over its own S columns
-__device__ __forceinline__ void umma_f16_ts_lh(uint32_t tmem_d, uint32_t tmem_a, uint32_t b_lo, uint32_t b_hi, uint32_t idesc,
-                                               uint32_t accumulate) {
-  asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      ".reg .b64 db;\n\t"
-      "setp.ne.b32 p, %5, 0;\n\t"
-      "mov.b64 db, {%2, %3};\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], db, %4, p;\n\t"
-      "}\n" ::"r"(tmem_d),
-      "r"(tmem_a), "r"(b_lo), "r"(b_hi), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-__device__ __forceinline__ void umma_commit_a(uint32_t bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
-}
-// a value every lane of a converged warp holds identically, made provably warp-uniform for the compiler (tcgen05
-// operands live in uniform registers; a value loaded from shared memory otherwise costs a broadcast loop per use)
-__device__ __forceinline__ uint32_t warp_uniform(uint32_t v) { return __shfl_sync(0xffffffffu, v, 0); }
-
-// ----------------------------------------------------------------------------------------------
-// tcgen05.ld / st: 32 lanes x 32 bit, N consecutive columns; thread i of the warp <-> TMEM lane
-// (warp_id % 4) * 32 + i.  taddr = (lane << 16) | column.
-// ----------------------------------------------------------------------------------------------
-__device__ __forceinline__ void tmem_ld_x32(uint32_t taddr, uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]),
-        "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]),
-        "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld_x16(uint32_t taddr, uint32_t (&r)[16]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_st_x16(uint32_t taddr, const uint32_t (&r)[16]) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x16.b32 [%0], "
-      "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16};" ::"r"(taddr),
-      "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]), "r"(r[8]), "r"(r[9]),
-      "r"(r[10]), "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15])
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-// The same wait, carrying the 32 destination registers of an EARLIER tmem_ld_x32 as read-write operands: every use of them
-// after this point depends on the wait, so the compiler cannot schedule one ahead of it (needed when other work sits between
-// the load and the wait — a software-pipelined epilogue).
-__device__ __forceinline__ void tmem_ld_wait_dep(uint32_t (&r)[32]) {
-  asm volatile("tcgen05.wait::ld.sync.aligned;"
-               : "+r"(r[0]), "+r"(r[1]), "+r"(r[2]), "+r"(r[3]), "+r"(r[4]), "+r"(r[5]), "+r"(r[6]), "+r"(r[7]), "+r"(r[8]),
-                 "+r"(r[9]), "+r"(r[10]), "+r"(r[11]), "+r"(r[12]), "+r"(r[13]), "+r"(r[14]), "+r"(r[15]), "+r"(r[16]),
-                 "+r"(r[17]), "+r"(r[18]), "+r"(r[19]), "+r"(r[20]), "+r"(r[21]), "+r"(r[22]), "+r"(r[23]), "+r"(r[24]),
-                 "+r"(r[25]), "+r"(r[26]), "+r"(r[27]), "+r"(r[28]), "+r"(r[29]), "+r"(r[30]), "+r"(r[31])
-               :
-               : "memory");
-}
-__device__ __forceinline__ void tmem_st_wait() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
 
 // Byte offset of 16-byte chunk `chunk16` (0..7) of row `row` inside a K-major SWIZZLE_128B tile whose
 // base is 1024-byte aligned and whose rows are 128 B (64 halfs).  Swizzle<3,4,3>: chunk ^= row % 8.
 __host__ __device__ __forceinline__ uint32_t sw128_offset(uint32_t row, uint32_t chunk16) {
   return row * 128u + (((chunk16 ^ (row & 7u)) & 7u) << 4);
-}
-
-// ----------------------------------------------------------------------------------------------
-// CTA pairs (cluster of 2, tcgen05 cta_group::2): one MMA spans the tensor cores of two SMs (M = 256); each CTA
-// stages its own 128 rows of A and HALF of the B tile, so per-SM shared-memory fill per FLOP drops by ~1/3.
-// ----------------------------------------------------------------------------------------------
-__device__ __forceinline__ uint32_t cluster_ctarank() {
-  uint32_t r;
-  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-  return r;
-}
-__device__ __forceinline__ void cluster_sync_all() {  // every thread of both CTAs
-  asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory");
-  asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-// shared::cluster address of `local_smem_addr` (a shared::cta address) in CTA `rank` of this cluster
-__device__ __forceinline__ uint32_t mapa_u32(uint32_t local_smem_addr, uint32_t rank) {
-  uint32_t r;
-  asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"(local_smem_addr), "r"(rank));
-  return r;
-}
-__device__ __forceinline__ void mbar_arrive_cluster(uint32_t cluster_addr) {
-  asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];" ::"r"(cluster_addr) : "memory");
-}
-__device__ __forceinline__ void tmem_alloc_pair(uint32_t* dst_smem, uint32_t ncols) {  // one warp in EACH CTA
-  asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(dst_smem)),
-               "r"(ncols)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc_pair(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-// D[tmem of both CTAs] (+)= A[128 rows in each CTA's smem] * B[N/2 rows in each CTA's smem]^T; leader CTA only
-__device__ __forceinline__ void umma_f16_ss_pair(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc,
-                                                 uint32_t accumulate) {
-  asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t"
-      "}\n" ::"r"(tmem_d),
-      "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// arrive (when the pair's MMAs issued so far retire) on the barrier at this smem offset in BOTH CTAs
-__device__ __forceinline__ void umma_commit_pair(uint64_t* bar) {
-  const uint16_t mask = 0x3;
-  asm volatile(
-      "tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(
-          smem_u32(bar)),
-      "h"(mask)
-      : "memory");
-}
-// TMA loads into MY shared memory whose completion is signalled on an mbarrier given by its shared::cluster address
-// (the leader CTA's barrier)
-__device__ __forceinline__ void tma_load_2d_pair(void* dst, const CUtensorMap* m, uint32_t bar_cluster_addr, int c0,
-                                                 int c1) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], "
-      "[%2];" ::"r"(smem_u32(dst)),
-      "l"(reinterpret_cast<uint64_t>(m)), "r"(bar_cluster_addr), "r"(c0), "r"(c1)
-      : "memory");
-}
-__device__ __forceinline__ void tma_load_4d_pair(void* dst, const CUtensorMap* m, uint32_t bar_cluster_addr, int c0,
-                                                 int c1, int c2, int c3) {
-  asm volatile(
-      "cp.async.bulk.tensor.4d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, "
-      "%6}], [%2];" ::"r"(smem_u32(dst)),
-      "l"(reinterpret_cast<uint64_t>(m)), "r"(bar_cluster_addr), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
-      : "memory");
 }
 
 // Same for a SWIZZLE_64B tile with 64-byte rows (32 halfs), chunk16 in 0..3.  Swizzle<2,4,3>: chunk ^= (row/2) % 4.

@@ -342,7 +342,7 @@ class SDEngine:
                  device="cuda:0", dtype=torch.float16, use_graphs: bool = True, vae_chunk: int = 8):
         self.device = torch.device(device)
         if self.device.type != "cuda" and self._require_cuda:
-            raise RuntimeError("SDEngine needs a CUDA device: the hot path is sm_100a kernels only (no CPU fallback)")
+            raise RuntimeError("SDEngine needs a CUDA device: the hot path is sm_90a kernels only (no CPU fallback)")
         self.dtype = dtype
         self.unet_cfg, self.vae_cfg, self.clip_cfg = unet_cfg, vae_cfg, clip_cfg
         self.use_graphs = use_graphs

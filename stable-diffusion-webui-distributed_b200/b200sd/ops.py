@@ -1,6 +1,6 @@
 """Thin torch-tensor wrappers over the C ABI (include/b200sd.h).
 
-torch is used for device memory and streams only; every op below launches hand-written sm_100a kernels
+torch is used for device memory and streams only; every op below launches hand-written sm_90a kernels
 from libb200sd.so on torch's current stream.  Tensors are NHWC / row-major; `ld`-style pitches come from
 `tensor.stride(-2)` so channel slices of wider buffers can be passed directly.
 """
@@ -63,14 +63,15 @@ def _epi(bias, bias_group_rows, residual, flags):
     return e
 
 
-NUM_SMS = 148
+NUM_SMS = 132  # H100 SXM
 
 
 def pick_block_n(n: int, geglu: bool = False, m: Optional[int] = None) -> int:
     """Tile width of the persistent GEMM.  Without `m` (and always for GEGLU, whose weights are interleaved per tile at
     pack time) the widest divisor of N; with `m`, the divisor that wastes the fewest SM-slots in the last wave of
-    ceil(M/128) * N/bn tiles over 148 SMs, with a mild preference for wide MMAs."""
-    cands = [bn for bn in (256, 192, 160, 128, 96, 64, 32) if n % bn == 0 and (not geglu or bn % 64 == 0)]
+    ceil(M/128) * N/bn tiles over NUM_SMS SMs, with a mild preference for wide MMAs.  Tiles wider than 160 columns are
+    never picked: their 64 x bn accumulator per warpgroup does not fit the register budget without spills."""
+    cands = [bn for bn in (160, 128, 96, 64, 32) if n % bn == 0 and (not geglu or bn % 64 == 0)]
     if not cands:
         raise ValueError(f"N={n} has no supported tile width")
     if geglu or m is None:
@@ -82,7 +83,7 @@ def pick_block_n(n: int, geglu: bool = False, m: Optional[int] = None) -> int:
             continue
         tiles = mt * (n // bn)
         waves = -(-tiles // NUM_SMS)
-        score = tiles / (waves * NUM_SMS) * (1.0 if bn >= 192 else 0.97 if bn >= 160 else 0.93)
+        score = tiles / (waves * NUM_SMS) * (1.0 if bn >= 160 else 0.97 if bn >= 128 else 0.93)
         if best is None or score > best[0] + 1e-9:
             best = (score, bn)
     return best[1]

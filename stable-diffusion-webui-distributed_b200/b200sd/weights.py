@@ -1,4 +1,4 @@
-"""Weight packing for the sm_100a kernels (one-time, at model load).
+"""Weight packing for the sm_90a kernels (one-time, at model load).
 
 Upstream (ldm) layouts -> kernel layouts:
   conv  [Cout, Cin, kh, kw]        -> [Cout, kh*kw*Cin]  (tap-major, channels innermost: matches NHWC im2col order)

@@ -2,7 +2,7 @@
 
 Drop-in for the reference's scripts/spartan/worker.py (`State` :36-41, `Worker` :51, `eta` :230-286,
 `request` :288-504, `benchmark` :506-575, `set_state` :719-758) with the same attributes and method signatures.
-`Worker` keeps the HTTP transport so an sdwui instance on another box can still be driven; the B200-native
+`Worker` keeps the HTTP transport so an sdwui instance on another box can still be driven; the GPU-native
 transport is `LocalGPUWorker` (local_worker.py), which overrides `request()` with an in-process executor.
 
 Conscious fixes of reference quirks (SURVEY.md App. E), everything else behaves identically:

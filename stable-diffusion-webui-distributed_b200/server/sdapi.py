@@ -1,4 +1,4 @@
-"""sdwui-compatible REST worker backed by the B200 executor (SURVEY.md §8 row f1).
+"""sdwui-compatible REST worker backed by the H100 executor (SURVEY.md §8 row f1).
 
 The reference reaches its workers only through nine sdwui API routes (SURVEY §2.2; all issued from
 scripts/spartan/worker.py and world.py of the reference):
@@ -13,7 +13,7 @@ scripts/spartan/worker.py and world.py of the reference):
     GET  /sdapi/v1/script-info                   world.py:750
 
 This module serves exactly those, with the reply shapes the reference reads, on top of `LocalGPUWorker` — so an
-UNMODIFIED reference master (or this repo's `Worker` with its HTTP transport) can list a B200 box in its
+UNMODIFIED reference master (or this repo's `Worker` with its HTTP transport) can list an H100 node in its
 `distributed-config.json` like any other sdwui node.  One process serves the GPUs of one box: requests are dispatched to
 the least-loaded device, one generation per device at a time (the executor replays CUDA graphs; the GIL is idle).
 

@@ -1,7 +1,7 @@
 """Minimal stand-in for the sdwui host modules, for running the worker server OUTSIDE sdwui.
 
 `scripts.spartan.{shared,worker,local_worker}` import `modules.shared` (cmd_opts, state) and
-`modules.initialize_util` because inside sdwui they are the plugin's host.  A B200 box that only serves the REST API
+`modules.initialize_util` because inside sdwui they are the plugin's host.  A GPU node that only serves the REST API
 has no sdwui: `install()` registers just those attributes — and nothing at all when a real `modules` package is
 importable (i.e. when this code runs as an sdwui extension).
 """

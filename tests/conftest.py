@@ -12,7 +12,7 @@ for p in (ROOT, EXT_DIR, HOSTSTUB):
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (B200); run with -m gpu on the GPU box")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (H100); run with -m gpu")
     try:   # fp32 references are IEEE fp32 on the GPU too (cuDNN's default lets fp32 convolutions use TF32 tensor cores)
         import torch
         torch.backends.cudnn.allow_tf32 = False

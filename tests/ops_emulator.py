@@ -43,7 +43,7 @@ def linear(a, wt, out, bias=None, bias_group_rows=0, residual=None, flags=0, blo
 
 
 def pick_block_n(n, geglu=False):
-    for bn in (256, 192, 160, 128, 96, 64, 32):
+    for bn in (160, 128, 96, 64, 32):
         if n % bn == 0 and (not geglu or bn % 64 == 0):
             return bn
     raise ValueError(n)

@@ -1,9 +1,11 @@
 """Drives a running sdwui-API worker server with the UNMODIFIED reference `Worker` class (/root/reference), in its own
 process because the reference's module names (`scripts.spartan.*`) are the same as this repo's.
 
-    python tests/ref_rest_probe.py <port>        -> one JSON line on stdout
+    REFERENCE_DIR=<reference checkout> python tests/ref_rest_probe.py <port>   -> one JSON line on stdout
 
-Used by tests/test_rest_worker_cpu.py when /root/reference exists (build container only).
+tests/golden/gen_ref_rest_golden.py runs it once against the REST server and stores what it saw (the HTTP exchanges
+and the values the reference Worker parsed out of them) in tests/golden/ref_rest_golden.json, which
+tests/test_rest_worker_cpu.py replays.
 """
 import base64
 import io
@@ -38,8 +40,28 @@ logging.getLogger("distributed").setLevel(logging.CRITICAL + 1)
 shared.benchmark_payload = pmodels.Benchmark_Payload()  # what World.load_config() installs (world.py:672-676)
 
 
+EXCHANGES = []  # every HTTP exchange the reference Worker makes: (method, path, JSON body) -> (status, JSON reply)
+
+
+def _recording(orig):
+    from urllib.parse import urlsplit
+
+    def request(self, method, url, *a, **k):
+        r = orig(self, method, url, *a, **k)
+        try:
+            reply = r.json()
+        except ValueError:
+            reply = None
+        EXCHANGES.append({"method": method.upper(), "path": urlsplit(url).path, "json": k.get("json"),
+                          "status": r.status_code, "reply": reply})
+        return r
+    return request
+
+
 def main():
     port = int(sys.argv[1])
+    import requests
+    requests.Session.request = _recording(requests.Session.request)
     w = worker.Worker(address="127.0.0.1", port=port, label="b200box", verify_remotes=False, avg_ipm=600.0)
     out = {"reference_file": worker.__file__, "reachable": bool(w.reachable())}
     w.benchmarked = True
@@ -60,6 +82,7 @@ def main():
                          for s in r["images"]]
     out["loaded_model"] = w.loaded_model
     out["models"] = w.available_models()
+    out["exchanges"] = EXCHANGES
     print(json.dumps(out))
 
 

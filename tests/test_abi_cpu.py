@@ -9,7 +9,7 @@ def test_library_exports_every_declared_symbol():
     lib = _lib.load()
     for n in names:
         assert hasattr(lib, n), n
-    assert lib.b200sd_version().decode().endswith("sm_100a")
+    assert lib.b200sd_version().decode().endswith("sm_90a")
 
 
 def test_missing_library_fails_loudly(tmp_path):

@@ -1,4 +1,4 @@
-"""The JSON lines bench.py printed on the B200 boxes (committed under profiles/) carry every key the measurement contract
+"""The JSON lines bench.py printed on the H100 (committed under profiles/) carry every key the measurement contract
 names, with consistent values — a schema regression in bench.py shows up here before a GPU visit is spent on it."""
 import glob
 import json
@@ -13,8 +13,7 @@ def _line(name):
     return json.loads(open(os.path.join(ROOT, "profiles", name)).read().strip().splitlines()[-1])
 
 
-@pytest.mark.parametrize("name", ["r02g_bench.json", "r02h_bench_n2.json", "r02h_bench_n4.json", "r02h_bench_n8.json",
-                                  "r02g_bench_img2img.json", "r02g_bench_sdxl.json", "r02j_bench_lean_rev1.json"])
+@pytest.mark.parametrize("name", ["h100_bench.json", "h100_bench_sdxl.json"])
 def test_gpu_arm_line(name):
     d = _line(name)
     for k in ("metric", "value", "unit", "n_gpus", "steps", "warmup", "ms_per_step", "higher_is_better", "scaling",
@@ -37,15 +36,6 @@ def test_gpu_arm_line(name):
     if d.get("cpu_baseline"):
         c = d["cpu_baseline"]
         assert c["kind"] in ("port", "reference") and c["cores"] >= 1 and c["unit"] == d["unit"] and c["sample"]
-
-
-def test_reference_arm_line():
-    d = _line("r02i_bench_reference_arm_box.json")
-    assert d["impl"] == "reference" and d["unit"] == "images/s" and d["higher_is_better"] is True
-    assert d["e2e"] == {"value": d["value"], "unit": d["unit"], "h2d_bytes_per_step": 0, "d2h_bytes_per_step": 0}
-    assert d["cpu_baseline"]["value"] == d["value"] and d["cpu_baseline"]["kind"] in ("port", "reference")
-    # a measured whole request, not a composition: time x steps fits the wall clock of the run
-    assert d["ms_per_step"] * d["steps"] / 1e3 <= d["wall_s"] * 1.01
 
 
 def test_bench_defaults_and_flags():

@@ -234,9 +234,8 @@ def test_attention(ops, b, heads, sq, skv, d, ones_col):
 
 @pytest.mark.parametrize("skv", [129, 192, 257, 321, 384, 385, 448, 520, 832])
 def test_attention_ring_lengths(ops, skv):
-    """ring mode (kv longer than two tiles) at every phase of the MMA loop's unroll-by-six and of the K/V/P rings:
-    3 .. 13 kv tiles, full and ragged last tiles — the producer's loads ride on the softmax warps' barrier, so an
-    off-by-one in a slot or parity shows up as a hang (the bounded waits trap) or as garbage"""
+    """kv longer than the K/V ring (3 .. 13 kv tiles, full and ragged last tiles): every slot is refilled at every ring
+    phase, so an off-by-one in a slot or parity shows up as a hang (the bounded waits trap) or as garbage"""
     b, heads, sq, d = 3, 8, 512, 40
     g = _gen(skv)
     d_pad = 64
@@ -251,8 +250,8 @@ def test_attention_ring_lengths(ops, skv):
 
 @pytest.mark.parametrize("ones_col", [False, True])
 def test_attention_growing_logits_forces_rescale(ops, ones_col):
-    """Keys ordered so that the row maximum keeps rising tile after tile by far more than 2^8: exercises the lazy-max
-    redo path (O rescale in TMEM) on every tile."""
+    """Keys ordered so that the row maximum keeps rising tile after tile by far more than 2^8: the running maximum and
+    the rescale of the O accumulator change on every tile."""
     g = _gen(99)
     b, heads, s, d, d_pad = 1, 2, 1024, 40, 64
     q = _padded_heads(b, s, heads, d, d_pad, g)

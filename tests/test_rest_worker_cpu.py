@@ -1,6 +1,7 @@
 """SURVEY §8 row f1: the sdwui-compatible REST worker (server/sdapi.py), driven over real HTTP by
  (1) this repo's `Worker` (which keeps the reference's HTTP transport for remote nodes), and
- (2) the UNMODIFIED reference `Worker` in a subprocess, when /root/reference exists (build container only).
+ (2) the UNMODIFIED reference `Worker`: its recorded HTTP exchanges with this server (tests/golden/ref_rest_golden.json)
+     are replayed.
 The executor is replaced by a deterministic double: this file tests the wire contract, not the arithmetic."""
 import base64
 import hashlib
@@ -8,8 +9,6 @@ import io
 import json
 import os
 import socket
-import subprocess
-import sys
 import threading
 import time
 import types
@@ -79,6 +78,13 @@ def server():
 def _decode(b64png):
     from PIL import Image
     return np.asarray(Image.open(io.BytesIO(base64.b64decode(b64png))))
+
+
+def strip_images(reply):
+    """`reply` with every base64 PNG of its "images" list replaced by the SHA-1 of the decoded pixels"""
+    if isinstance(reply, dict) and isinstance(reply.get("images"), list):
+        reply = dict(reply, images=[hashlib.sha1(_decode(s).tobytes()).hexdigest() for s in reply["images"]])
+    return reply
 
 
 PAYLOAD = {"prompt": "a probe", "negative_prompt": "", "seed": 31, "subseed": 7, "subseed_strength": 0, "batch_size": 2,
@@ -205,17 +211,28 @@ def test_requests_are_bounded_and_restart_waits_for_the_running_generation():
     assert evicted == [True]            # the restart ran after the generation had been released
 
 
-@pytest.mark.skipif(not os.path.isdir(os.environ.get("REFERENCE_DIR", "/root/reference")),
-                    reason="the unmodified reference exists in the build container only")
-def test_unmodified_reference_worker_drives_the_rest_server(server):
+GOLDEN = os.path.join(HERE, "golden", "ref_rest_golden.json")
+
+
+def test_unmodified_reference_worker_exchanges_replay(server):
+    """What the UNMODIFIED reference `Worker` sent to and parsed from this server (recorded over real HTTP by
+    tests/golden/gen_ref_rest_golden.py), replayed: every request gets the recorded status and reply (the memory report
+    describes the host, so only its fields are compared), and what the reference parsed is what the server produces."""
+    import requests
     port, eng = server
-    p = subprocess.run([sys.executable, os.path.join(HERE, "ref_rest_probe.py"), str(port)], capture_output=True, text=True,
-                       timeout=120)
-    assert p.returncode == 0, p.stderr[-2000:]
-    out = json.loads(p.stdout.strip().splitlines()[-1])
-    assert out["reference_file"].startswith(os.environ.get("REFERENCE_DIR", "/root/reference"))
-    assert out["reachable"] and out["state"] == "IDLE" and out["n_images"] == 2
-    assert out["all_seeds"] == [31, 32] and out["all_subseeds"] == [7, 8]
+    g = json.load(open(GOLDEN))
+    assert g["reachable"] and g["state"] == "IDLE" and g["n_images"] == 2
+    assert g["all_seeds"] == [31, 32] and g["all_subseeds"] == [7, 8]
     want = _expected(eng, PAYLOAD)
-    assert out["image_sha1"] == [hashlib.sha1(want[i].numpy().tobytes()).hexdigest() for i in range(2)]
-    assert out["loaded_model"] == "m.safetensors" and len(out["models"]) == 1
+    assert g["image_sha1"] == [hashlib.sha1(want[i].numpy().tobytes()).hexdigest() for i in range(2)]
+    assert g["loaded_model"] == "m.safetensors" and len(g["models"]) == 1
+    assert [ex["path"] for ex in g["exchanges"]] == ["/sdapi/v1/memory", "/sdapi/v1/memory", "/sdapi/v1/options",
+                                                     "/sdapi/v1/txt2img", "/sdapi/v1/sd-models"]
+    for ex in g["exchanges"]:
+        r = requests.request(ex["method"], f"http://127.0.0.1:{port}{ex['path']}", json=ex["json"], timeout=60)
+        assert r.status_code == ex["status"], ex["path"]
+        got = strip_images(r.json())
+        if ex["path"] == "/sdapi/v1/memory":
+            assert set(got) == set(ex["reply"]) and set(got["ram"]) == set(ex["reply"]["ram"]), got
+        else:
+            assert got == ex["reply"], ex["path"]
