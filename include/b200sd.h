@@ -47,10 +47,6 @@ typedef struct b200sd_epilogue {
 
 /* library / build identification: returns a static string "b200sd <version> sm_90a" */
 const char* b200sd_version(void);
-/* debug hooks kept for ABI compatibility: the sm_90a attention and GEMM / conv kernels record no timeline, so the buffer is
- * never written; both return 0. */
-int b200sd_debug_attention_trace(void* device_buffer);
-int b200sd_debug_gemm_trace(void* device_buffer);
 
 /* ---- tensor-core ops (wgmma + TMA) -------------------------------------------------------------- */
 
@@ -90,22 +86,11 @@ int b200sd_groupnorm_stats(const void* X, long long pitch, int NB, int HW, int C
 int b200sd_groupnorm_apply(const void* X, long long pitch_x, void* Y, long long pitch_y, int NB, int HW, int C, int G,
                            const float* stats, const float* gamma, const float* beta, float eps, int silu, int dtype,
                            void* stream);
-/* GroupNorm in one call.  mode 1: b200sd_groupnorm_stats + b200sd_groupnorm_apply.  mode 2: the one-pass kernel — each CTA
- * keeps its ~48 KB slab of an image in shared memory while the image's CTAs agree on the statistics (1 read + 1 write
- * instead of 2 reads + 1 write) — or B200SD_ERR_UNSUPPORTED when the shape is not eligible (C <= 2048, G <= 64 and all
- * slabs of ONE image resident on the device at the same time: a function of HW and C only, never of NB, so an image's bits
- * do not depend on the batch it travels in).  mode 0: mode 1, unless B200SD_GN_FUSED=1 and the shape is eligible (the
- * cross-CTA agreement of the one-pass kernel can cost more than the second read it saves, DESIGN.md section 4).  `stats` as
- * for b200sd_groupnorm_stats. */
+/* GroupNorm in one call: b200sd_groupnorm_stats, then b200sd_groupnorm_apply on the same stream.  How the pixels of an
+ * image are split between CTAs depends on HW and C only, never on NB, so an image's bits do not depend on the batch it
+ * travels in.  `stats` as for b200sd_groupnorm_stats. */
 int b200sd_groupnorm(const void* X, long long pitch_x, void* Y, long long pitch_y, int NB, int HW, int C, int G,
-                     float* stats, const float* gamma, const float* beta, float eps, int silu, int mode, int dtype,
-                     void* stream);
-/* 1 if modes 0 / 2 take the one-pass kernel for this shape on the current device. */
-int b200sd_groupnorm_is_fused(int NB, int HW, int C, int G, int dtype);
-/* measurement aid: slab KB of the one-pass kernel, 8..160 (0 = keep; default 48, env
- * B200SD_GN_FUSED_KB) — call b200sd_groupnorm_stats_floats again afterwards — and whether the statistics kernel walks the
- * tensor back to front (-1 = keep; default 1, env B200SD_GN_REVERSE). */
-int b200sd_debug_gn_config(int slab_kb, int reverse_stats);
+                     float* stats, const float* gamma, const float* beta, float eps, int silu, int dtype, void* stream);
 /* LayerNorm over the last dim of [rows, C]. (upstream BasicTransformerBlock.norm1/2/3) */
 int b200sd_layernorm(const void* X, long long ldx, void* Y, long long ldy, int rows, int C, const float* gamma,
                      const float* beta, float eps, int dtype, void* stream);

@@ -312,9 +312,3 @@ int attention_tc(const void* Q, long long ldq, const void* K, long long ldk, con
 }
 
 }  // namespace b200sd
-
-// debug hook kept for ABI compatibility: the sm_90a attention kernel records no timeline, so the buffer is never written
-extern "C" int b200sd_debug_attention_trace(void* device_buffer) {
-  (void)device_buffer;
-  return B200SD_OK;
-}

@@ -586,9 +586,3 @@ int conv_tc(const void* X, long long pitch_c, int NB, int Hin, int Win, int C, c
 }
 
 }  // namespace b200sd
-
-// debug hook kept for ABI compatibility: the sm_90a GEMM / conv kernel records no timeline, so the buffer is never written
-extern "C" int b200sd_debug_gemm_trace(void* device_buffer) {
-  (void)device_buffer;
-  return B200SD_OK;
-}

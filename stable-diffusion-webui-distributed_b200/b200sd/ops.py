@@ -160,40 +160,20 @@ def groupnorm_stats_floats(nb: int, hw: int, c: int, groups: int) -> int:
     return n
 
 
-_GN_FUSED = {}
-
-
-def groupnorm_is_fused(nb: int, hw: int, c: int, groups: int, dtype) -> bool:
-    """whether the ONE-PASS GroupNorm kernel can take this shape on the current device (groupnorm(mode=2))"""
-    key = (hw, c, groups, dtype, torch.cuda.current_device())
-    if key not in _GN_FUSED:
-        code = BF16 if dtype == torch.bfloat16 else F16
-        _GN_FUSED[key] = bool(_lib.lib().b200sd_groupnorm_is_fused(nb, hw, c, groups, code))
-    return _GN_FUSED[key]
-
-
-def groupnorm_one_pass_default(nb: int, hw: int, c: int, groups: int, dtype) -> bool:
-    """whether groupnorm(mode=0) runs as one kernel: only with B200SD_GN_FUSED=1 (measured slower than statistics + apply
-    at the UNet's shapes, DESIGN.md section 4) and an eligible shape"""
-    import os
-    return os.environ.get("B200SD_GN_FUSED", "0") not in ("0", "") and groupnorm_is_fused(nb, hw, c, groups, dtype)
-
-
 def groupnorm(x: torch.Tensor, out: torch.Tensor, stats: torch.Tensor, gamma: torch.Tensor, beta: torch.Tensor,
-              groups: int, eps: float, silu: bool, mode: int = 0):
+              groups: int, eps: float, silu: bool):
     """x, out [NB, HW, C] (pitch = stride(1)); stats: flat fp32 buffer of groupnorm_stats_floats(...) elements,
     zero-filled once at allocation (may be shared by successive calls on one stream); its first NB*groups*2 elements
-    receive (sum, sumsq) per (image, group) — deterministically, run to run.  mode: 0 the library's default (statistics +
-    apply kernels unless B200SD_GN_FUSED=1), 1 statistics + apply, 2 the one-pass kernel or an error (include/b200sd.h)."""
+    receive (sum, sumsq) per (image, group) — deterministically, run to run.  Two launches: statistics, then apply."""
     nb, hw, c = x.shape
     assert x.stride(2) == 1 and out.stride(2) == 1 and x.stride(0) == hw * x.stride(1)
     assert stats.dtype == torch.float32 and stats.is_contiguous()
     assert stats.numel() >= groupnorm_stats_floats(nb, hw, c, groups), "stats buffer too small"
     rc = _lib.lib().b200sd_groupnorm(_p(x), ctypes.c_longlong(x.stride(1)), _p(out), ctypes.c_longlong(out.stride(1)), nb,
                                      hw, c, groups, _p(stats), _p(gamma), _p(beta), ctypes.c_float(eps), int(silu),
-                                     int(mode), _dt(x), _stream())
+                                     _dt(x), _stream())
     check(rc, "b200sd_groupnorm")
-    _count(1 if mode == 2 or (mode == 0 and groupnorm_one_pass_default(nb, hw, c, groups, x.dtype)) else 2)
+    _count(2)
     return out
 
 

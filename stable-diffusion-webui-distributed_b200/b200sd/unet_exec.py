@@ -205,7 +205,6 @@ class UNetProgram:
         self.ops: List = []
         self.op_flops: List = []
         self.gn_elems = self.ln_elems = 0     # elements normalised per evaluation (bench.py's HBM roofline)
-        self.gn_fused_elems = 0               # ... of which through the one-pass GroupNorm kernel (4 instead of 6 B / element)
         self._build()
         # one statistics buffer serves every GroupNorm (they run back to back on one stream); zeroed once, here
         self.stats_all = torch.zeros((max(1, self.gn_need),), device=self.dev, dtype=torch.float32)
@@ -234,9 +233,6 @@ class UNetProgram:
         self.gn_need = max(self.gn_need, ops.groupnorm_stats_floats(x.shape[0], x.shape[1], x.shape[2], 32))
         g, b = self.w.t[name + ".g"], self.w.t[name + ".beta"]
         self.gn_elems += x.shape[0] * x.shape[1] * x.shape[2]
-        one_pass = getattr(ops, "groupnorm_one_pass_default", None)   # absent from the CPU emulation of ops used by the host tests
-        if one_pass is not None and x.is_cuda and one_pass(x.shape[0], x.shape[1], x.shape[2], 32, x.dtype):
-            self.gn_fused_elems += x.shape[0] * x.shape[1] * x.shape[2]
         self._emit(lambda: ops.groupnorm(x, out, holder[0], g, b, 32, eps, silu))
 
     def _res(self, key, x, cin, cout, h, wd, dest):

@@ -87,7 +87,7 @@ def groupnorm_stats_floats(nb, hw, c, groups):
     return nb * groups * 2
 
 
-def groupnorm(x, out, stats, gamma, beta, groups, eps, silu, mode=0):
+def groupnorm(x, out, stats, gamma, beta, groups, eps, silu):
     y = F.group_norm(x.float().permute(0, 2, 1), groups, gamma, beta, eps).permute(0, 2, 1)
     if silu:
         y = F.silu(y)
