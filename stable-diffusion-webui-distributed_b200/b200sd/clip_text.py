@@ -7,6 +7,9 @@ kernel scope ("run in torch").
   * SDXL (sgm GeneralConditioner, sd_xl_base.yaml): the CLIP-L tower read at hidden layer 11 (no final LN) next to an
     OpenCLIP ViT-bigG tower (penultimate layer; pooled = ln_final(last)[EOS] @ text_projection), and the vector
     conditioning cat(pooled, Fourier features of original size, crop, target size) that feeds the UNet's label_emb.
+  * Prompts longer than one chunk (sdwui FrozenCLIPEmbedderWithCustomWordsBase): tokens [B, 77 * k] are k separate
+    77-token sequences through the tower, concatenated along the tokens; emphasis multipliers scale each chunk's output
+    as sdwui's EmphasisOriginal does.
 """
 import math
 import threading
@@ -22,8 +25,19 @@ CAPTURE_LOCK = threading.Lock()   # CUDA graph captures are serialised across th
 
 
 class Cond(NamedTuple):
-    ctx: torch.Tensor                 # [B, 77, context_dim] cross-attention context
+    ctx: torch.Tensor                 # [B, 77 * k, context_dim] cross-attention context
     y: Optional[torch.Tensor] = None  # [B, adm_in_channels] vector conditioning (SDXL), or None
+
+
+def emphasis(z: torch.Tensor, mult: torch.Tensor) -> torch.Tensor:
+    """sdwui EmphasisOriginal on one chunk of one prompt: z [77, W] tower output, mult [77]: z * m, rescaled so that the
+    mean over the chunk's 77 x W values is what it was; fp32 math.  One sequence per call, so the reductions have the
+    same shape whatever the batch (a batched mean may sum in another order)."""
+    zf = z.float()
+    before = zf.mean()
+    zf = zf * mult.to(device=z.device, dtype=torch.float32)[:, None]
+    zf = zf * (before / zf.mean())
+    return zf.to(z.dtype)
 
 
 def _attend(q, k, v, mask):
@@ -179,15 +193,40 @@ class Conditioner:
             return tuple(r.clone() for r in res)
 
     @torch.no_grad()
-    def __call__(self, tokens: torch.Tensor, width: int = 512, height: int = 512, zero_txt: bool = False) -> Cond:
-        """zero_txt (SDXL): sdwui's force_zero_embeddings=['txt'] for an all-empty negative prompt"""
+    def __call__(self, tokens: torch.Tensor, width: int = 512, height: int = 512, zero_txt: bool = False,
+                 multipliers: Optional[torch.Tensor] = None) -> Cond:
+        """tokens [B, 77 * k]; multipliers [B, 77 * k] emphasis weights (None or all 1: none applied).
+        zero_txt (SDXL): sdwui's force_zero_embeddings=['txt'] for an all-empty negative prompt"""
+        b, n = tokens.shape
+        if n % 77:
+            raise ValueError(f"prompt tokens must come in chunks of 77, got {n}")
+        k = n // 77
+        if multipliers is not None:
+            if tuple(multipliers.shape) != (b, n):
+                raise ValueError(f"multipliers {tuple(multipliers.shape)} do not match tokens {(b, n)}")
+            if bool((multipliers == 1.0).all()):
+                multipliers = None
+        seqs = tokens.reshape(b * k, 77)   # sequence i * k + j = chunk j of prompt i
+        first = None
+        if multipliers is not None:   # each distinct (tokens, multipliers) sequence is weighted once
+            mult = multipliers.reshape(b * k, 77).cpu().float()
+            keys = [(tuple(t), tuple(m)) for t, m in zip(seqs.cpu().tolist(), mult.tolist())]
+            seen = {}
+            first = [seen.setdefault(key, i) for i, key in enumerate(keys)]
+
+        def ctx_of(z):   # [b * k, 77, W] tower output -> emphasis -> [b, 77 * k, W]
+            if first is not None:
+                done = {i: emphasis(z[i], mult[i]) for i in sorted(set(first))}
+                z = torch.stack([done[i] for i in first])
+            return z.reshape(b, n, z.shape[-1])
+
         if not self.xl:
-            return Cond(self._chunked("t0", self.t0, tokens)[0])
+            return Cond(ctx_of(self._chunked("t0", self.t0, seqs)[0]))
         cfg = self.cfg
-        b = tokens.shape[0]
-        (h0,) = self._chunked("t0_hidden", lambda t: self.t0.hidden(t, cfg.layers - 1), tokens)
-        h1, pooled = self._chunked("t1", self.t1, tokens)
-        ctx = torch.cat([h0, h1], dim=-1)
+        (h0,) = self._chunked("t0_hidden", lambda t: self.t0.hidden(t, cfg.layers - 1), seqs)
+        h1, pooled = self._chunked("t1", self.t1, seqs)
+        pooled = pooled.reshape(b, k, -1)[:, 0]   # sdwui: the pooled vector of the first chunk, unweighted
+        ctx = torch.cat([ctx_of(h0), ctx_of(h1)], dim=-1)
         if zero_txt:
             ctx, pooled = torch.zeros_like(ctx), torch.zeros_like(pooled)
         scal = torch.tensor([height, width, 0, 0, height, width], dtype=torch.float32, device=self.device)

@@ -17,6 +17,15 @@ extern "C" int b200sd_conv2d(const void* X, long long pitch_c, int NB, int Hin, 
 extern "C" int b200sd_attention(const void* Q, long long ldq, const void* K, long long ldk, const void* V,
                                 long long ldv, void* O, long long ldo, int B, int heads, int Sq, int Skv, int d,
                                 int d_pad, float scale, int v_ones_col, int dtype, void* stream) {
-  return b200sd::attention_tc(Q, ldq, K, ldk, V, ldv, O, ldo, B, heads, Sq, Skv, d, d_pad, scale, v_ones_col,
+  return b200sd::attention_tc(Q, ldq, K, ldk, V, ldv, O, ldo, B, heads, Sq, Skv, nullptr, d, d_pad, scale, v_ones_col,
+                              dtype == B200SD_BF16 ? 1 : 0, static_cast<cudaStream_t>(stream));
+}
+
+extern "C" int b200sd_attention_varlen(const void* Q, long long ldq, const void* K, long long ldk, const void* V,
+                                       long long ldv, void* O, long long ldo, int B, int heads, int Sq, int Skv,
+                                       const int* kv_len, int d, int d_pad, float scale, int v_ones_col, int dtype,
+                                       void* stream) {
+  if (!kv_len) return B200SD_ERR_INVALID;
+  return b200sd::attention_tc(Q, ldq, K, ldk, V, ldv, O, ldo, B, heads, Sq, Skv, kv_len, d, d_pad, scale, v_ones_col,
                               dtype == B200SD_BF16 ? 1 : 0, static_cast<cudaStream_t>(stream));
 }

@@ -20,6 +20,13 @@
 //                    and B = V MN-major in shared memory
 // The row sums are accumulated in fp32 registers, so the ones column a caller may place in V (v_ones_col) is not needed
 // and its output column is not stored.
+//
+// Varlen mode (b200sd_attention_varlen, kVarlen): batch row b attends to keys [0, kv_len[b]) of a K/V buffer that is Skv
+// rows long; kv_len is a device array, so one captured graph serves any split of lengths.  A CTA walks only the
+// ceil(kv_len[b] / 64) tiles it needs and masks columns >= kv_len[b] as the ragged tail of a plain call.  Tile walk and
+// reduction order are those of a plain call with Skv = kv_len[b], so the results are bitwise equal to it as long as the
+// buffer rows in [kv_len[b], 64 * ceil(kv_len[b] / 64)) hold finite values (they get P = 0, where a plain call reads
+// the tensor map's zero fill).
 #include <cstddef>
 #include <cstdlib>
 
@@ -45,6 +52,7 @@ struct AttnParams {
   float scale_log2;  // softmax scale * log2(e)
   void* O;
   long long ldo;
+  const int* kv_len;  // varlen: [B] key counts on the device, clamped to [1, Skv]
 };
 
 struct __align__(8) AttnShared {
@@ -64,7 +72,7 @@ __device__ __forceinline__ uint32_t pack_h2(float a, float b) {
   }
 }
 
-template <int kChunks, bool kBf16>
+template <int kChunks, bool kBf16, bool kVarlen>
 __global__ void __launch_bounds__(kAttnThreads, 1)
 attention_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
                     const __grid_constant__ CUtensorMap tmV, const AttnParams p) {
@@ -84,7 +92,6 @@ attention_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_consta
   const int qt = blockIdx.x;
   const int head = blockIdx.y;
   const int b = blockIdx.z;
-  const int nkv = (p.Skv + kKv - 1) / kKv;
   const int col0 = head * p.d_pad;
   const bool loader = threadIdx.x == 0;
 
@@ -101,6 +108,8 @@ attention_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_consta
   }
   __syncthreads();
   pdl_wait();  // Q / K / V come from the preceding projection GEMM
+  const int skv = kVarlen ? min(max(p.kv_len[b], 1), p.Skv) : p.Skv;  // keys this batch row attends to
+  const int nkv = (skv + kKv - 1) / kKv;
 
   auto load_kv = [&](int t) {  // tile t into slot t % stages (the slot is free)
     const int s = t % p.stages;
@@ -151,8 +160,8 @@ attention_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_consta
     wgmma_wait<0>();
     reg_fence(sacc);
 
-    // online softmax (scaled logits in log2 units); kv columns >= Skv are masked
-    const int valid = p.Skv - t * kKv;
+    // online softmax (scaled logits in log2 units); kv columns >= skv are masked
+    const int valid = skv - t * kKv;
     float mx[2] = {-INFINITY, -INFINITY};
 #pragma unroll
     for (int g = 0; g < 8; ++g)
@@ -226,14 +235,15 @@ attention_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_consta
 // ------------------------------------------------------------------------------------------------
 typedef void (*AttnKernel)(CUtensorMap, CUtensorMap, CUtensorMap, AttnParams);
 
+template <bool kVarlen>
 static AttnKernel attn_kernel_for(int chunks, int is_bf16) {
   switch (chunks * 2 + (is_bf16 ? 1 : 0)) {
-    case 2: return attention_tc_kernel<1, false>;
-    case 3: return attention_tc_kernel<1, true>;
-    case 4: return attention_tc_kernel<2, false>;
-    case 5: return attention_tc_kernel<2, true>;
-    case 6: return attention_tc_kernel<3, false>;
-    case 7: return attention_tc_kernel<3, true>;
+    case 2: return attention_tc_kernel<1, false, kVarlen>;
+    case 3: return attention_tc_kernel<1, true, kVarlen>;
+    case 4: return attention_tc_kernel<2, false, kVarlen>;
+    case 5: return attention_tc_kernel<2, true, kVarlen>;
+    case 6: return attention_tc_kernel<3, false, kVarlen>;
+    case 7: return attention_tc_kernel<3, true, kVarlen>;
     default: return nullptr;
   }
 }
@@ -242,8 +252,8 @@ static int g_attn_max_smem = 0;
 static bool g_attn_dev_ready[64] = {};
 
 int attention_tc(const void* Q, long long ldq, const void* K, long long ldk, const void* V, long long ldv, void* O,
-                 long long ldo, int B, int heads, int Sq, int Skv, int d, int d_pad, float scale, int v_ones_col,
-                 int is_bf16, cudaStream_t stream) {
+                 long long ldo, int B, int heads, int Sq, int Skv, const int* kv_len, int d, int d_pad, float scale,
+                 int v_ones_col, int is_bf16, cudaStream_t stream) {
   if (B <= 0 || heads <= 0 || Sq <= 0) return B200SD_OK;
   // d_pad: the head pitch in Q / K / V, a multiple of 16
   if (Skv <= 0 || d <= 0 || d % 8 != 0 || d_pad % 16 != 0 || d_pad < d) return B200SD_ERR_INVALID;
@@ -255,6 +265,7 @@ int attention_tc(const void* Q, long long ldq, const void* K, long long ldk, con
       ldv < static_cast<long long>(heads) * d_pad || ldo < static_cast<long long>(heads) * d)
     return B200SD_ERR_INVALID;
   if (v_ones_col && d >= d_pad) return B200SD_ERR_INVALID;  // the ones column needs a free pad column
+  if (kv_len && (reinterpret_cast<uintptr_t>(kv_len) & 3)) return B200SD_ERR_INVALID;
   const int chunks = (d_pad + 63) / 64;
   if (chunks > 3) return B200SD_ERR_UNSUPPORTED;
   {
@@ -267,8 +278,10 @@ int attention_tc(const void* Q, long long ldq, const void* K, long long ldk, con
         return B200SD_ERR_CUDA;
       for (int c = 1; c <= 3; ++c)
         for (int bf = 0; bf < 2; ++bf)
-          if (cudaFuncSetAttribute(attn_kernel_for(c, bf), cudaFuncAttributeMaxDynamicSharedMemorySize, smem) !=
-              cudaSuccess)
+          if (cudaFuncSetAttribute(attn_kernel_for<false>(c, bf), cudaFuncAttributeMaxDynamicSharedMemorySize, smem) !=
+                  cudaSuccess ||
+              cudaFuncSetAttribute(attn_kernel_for<true>(c, bf), cudaFuncAttributeMaxDynamicSharedMemorySize, smem) !=
+                  cudaSuccess)
             return B200SD_ERR_CUDA;
       g_attn_max_smem = smem;
       g_attn_dev_ready[dev] = true;
@@ -280,6 +293,7 @@ int attention_tc(const void* Q, long long ldq, const void* K, long long ldk, con
   p.chunks = chunks;
   p.scale_log2 = scale * 1.4426950408889634f;
   p.O = O; p.ldo = ldo;
+  p.kv_len = kv_len;
   const int nkv = (Skv + kKv - 1) / kKv;
   const size_t qt = static_cast<size_t>(chunks) * kQChunkBytes;
   const size_t kvt = 2 * static_cast<size_t>(chunks) * kKvChunkBytes;  // K and V of one slot
@@ -307,7 +321,7 @@ int attention_tc(const void* Q, long long ldq, const void* K, long long ldk, con
     if ((rc = make_tmap_sw128(&tmV, V, 3, dims, st, kvbox, es)) != B200SD_OK) return rc;
   }
   dim3 grid((Sq + kQTile - 1) / kQTile, heads, B);
-  launch_pdl(attn_kernel_for(chunks, is_bf16), grid, dim3(kAttnThreads), smem, stream, tmQ, tmK, tmV, p);
+  launch_pdl(kv_len ? attn_kernel_for<true>(chunks, is_bf16) : attn_kernel_for<false>(chunks, is_bf16), grid, dim3(kAttnThreads), smem, stream, tmQ, tmK, tmV, p);
   return cudaGetLastError() == cudaSuccess ? B200SD_OK : B200SD_ERR_CUDA;
 }
 

@@ -13,7 +13,7 @@ int conv_tc(const void* X, long long pitch_c, int NB, int Hin, int Win, int C, c
             int is_bf16, int max_ctas, cudaStream_t stream);
 
 int attention_tc(const void* Q, long long ldq, const void* K, long long ldk, const void* V, long long ldv, void* O,
-                 long long ldo, int B, int heads, int Sq, int Skv, int d, int d_pad, float scale, int v_ones_col,
-                 int is_bf16, cudaStream_t stream);
+                 long long ldo, int B, int heads, int Sq, int Skv, const int* kv_len, int d, int d_pad, float scale,
+                 int v_ones_col, int is_bf16, cudaStream_t stream);
 
 }  // namespace b200sd

@@ -22,6 +22,7 @@ from .vae_exec import VAEDecoderProgram, VAEDecoderWeights, VAEEncoderProgram, V
 MAX_STEPS = 256
 MAX_PLANS = 6        # distinct (batch, latent h, w) kept per engine; the least recently used one is dropped beyond that
 MAX_GRAPHS = 48      # step graphs kept per plan (one per sampler stage structure x cfg scale): oldest dropped beyond that
+CHUNK = 77           # tokens per prompt chunk (sdwui: [BOS] + 75 + [EOS]); contexts are 77 * k tokens long
 NOISE_SAMPLERS = ("Euler a", "stage")   # graph-name prefixes of the step graphs that may read Plan.noise
 # _CAPTURE_LOCK (imported): CUDA graph captures are serialised across the per-device worker threads
 
@@ -247,7 +248,8 @@ class Plan:
     def __init__(self, eng: "SDEngine", b: int, h: int, w: int, vae_chunk: int):
         dev = eng.device
         self.b, self.h, self.w = b, h, w
-        self.unet = UNetProgram(eng.unet_w, 2 * b, h, w)
+        self.unet = UNetProgram(eng.unet_w, 2 * b, h, w, CHUNK)
+        self.kv_len = self.unet.kv_len   # int32 [2b] on the device: context tokens of every [cond | uncond] row
         self.vae_chunk = min(vae_chunk, b)
         self.vae = VAEDecoderProgram(eng.vae_w, self.vae_chunk, h, w)
         self.x = torch.zeros((b, h * w, 4), device=dev, dtype=torch.float32)
@@ -280,6 +282,34 @@ class Plan:
                 del self.graphs[name]
                 self.graph_launches.pop(name, None)
         return self.noise
+
+    @property
+    def ctx_cap(self) -> int:
+        """context capacity: rows per image of the cross-attention K/V buffers (a multiple of 77)"""
+        return self.unet.ctx_len
+
+    def ensure_context(self, tokens: int):
+        """grow the K/V buffers in whole 77-token chunks to hold a `tokens`-long context; growing drops the step graphs
+        that captured the old buffers (the "vae" graph does not read them).  Activation buffers are not duplicated."""
+        if tokens > self.ctx_cap:
+            self.unet.grow_context(-(-tokens // CHUNK) * CHUNK)
+            for name in [n for n in self.graphs if n != "vae"]:
+                del self.graphs[name]
+                self.graph_launches.pop(name, None)
+
+    def set_context(self, cond_ctx: torch.Tensor, uncond_ctx: torch.Tensor):
+        """[cond | uncond] contexts -> the UNet's cross-attention K/V.  Equal lengths take the plain batched call; different
+        lengths (sdwui then runs two UNet calls) are zero-padded to the longer one and attend to their own lengths."""
+        b, lc, c = cond_ctx.shape
+        lu = uncond_ctx.shape[1]
+        self.ensure_context(max(lc, lu))
+        if lc == lu:
+            self.unet.set_context(torch.cat([cond_ctx, uncond_ctx]).to(self.unet.dt).contiguous())
+            return
+        ctx = torch.zeros((2 * b, max(lc, lu), c), device=self.x.device, dtype=self.unet.dt)
+        ctx[:b, :lc] = cond_ctx
+        ctx[b:, :lu] = uncond_ctx
+        self.unet.set_context(ctx, [lc] * b + [lu] * b)
 
     # one sampler step = select this step's biases, UNet on [cond | uncond], CFG + update + repack
     def step_ddim(self, cfg_scale: float):
@@ -399,17 +429,22 @@ class SDEngine:
                 torch.cuda.empty_cache()
 
     @torch.no_grad()
-    def encode_prompts(self, tokens: torch.Tensor, width: int = 512, height: int = 512, zero_txt: bool = False):
-        """tokens [b, 77] -> cross-attention context [b, 77, ctx] (SD1.x), or Cond(ctx, vector conditioning) for SDXL"""
+    def encode_prompts(self, tokens: torch.Tensor, width: int = 512, height: int = 512, zero_txt: bool = False,
+                       multipliers: Optional[torch.Tensor] = None):
+        """tokens [b, 77 * k] (k chunks of [BOS] + 75 + [EOS], factory.tokenize_prompts) -> cross-attention context
+        [b, 77 * k, ctx] (SD1.x), or Cond(ctx, vector conditioning) for SDXL.  multipliers [b, 77 * k]: sdwui emphasis
+        weights of the tokens (None: all 1)."""
         with self._ctx():
-            c = self.clip(tokens, width, height, zero_txt)
+            c = self.clip(tokens, width, height, zero_txt, multipliers)
             return c if c.y is not None else c.ctx
 
-    def _conds(self, tokens: torch.Tensor, neg_tokens: torch.Tensor, width: int, height: int):
+    def _conds(self, tokens: torch.Tensor, neg_tokens: torch.Tensor, width: int, height: int, multipliers=None,
+               neg_multipliers=None):
         """(cond, uncond) of a request.  SDXL: an all-empty negative prompt ([BOS] + EOS padding in every row) gets zero
         text embeddings, as sdwui's sd_models_xl.get_learned_conditioning does (force_zero_embeddings=['txt'])."""
         empty_neg = self.clip.xl and bool((neg_tokens[:, 1:] == neg_tokens[:, -1:]).all())
-        return (self.encode_prompts(tokens, width, height), self.encode_prompts(neg_tokens, width, height, zero_txt=empty_neg))
+        return (self.encode_prompts(tokens, width, height, multipliers=multipliers),
+                self.encode_prompts(neg_tokens, width, height, zero_txt=empty_neg, multipliers=neg_multipliers))
 
     def _graph(self, plan: Plan, name: str, fn):
         """Run fn eagerly once (per-device kernel attribute setup must not happen under capture), then capture."""
@@ -516,7 +551,7 @@ class SDEngine:
     @torch.no_grad()
     def run_program(self, cond: torch.Tensor, uncond: torch.Tensor, x_start: torch.Tensor, pr: "Program", cfg_scale: float,
                     noises: Optional[torch.Tensor] = None, inpaint=None) -> torch.Tensor:
-        """cond/uncond [b, 77, ctx] on device; x_start [b, 4, h, w] fp32 (host or device) = Program.start(...): the start
+        """cond/uncond [b, 77 * k, ctx] on device (cond and uncond may have different k); x_start [b, 4, h, w] fp32 (host or device) = Program.start(...): the start
         latents in the sampler's own space; noises [pr.draws, b, 4, h, w]: the per-image N(0,1) draws after the first;
         inpaint = (clean init latents [b, 4, h, w], latent mask [h * w]).  Returns the final latents fp32 [b, h*w, 4]
         (NHWC, a view of plan state)."""
@@ -530,7 +565,7 @@ class SDEngine:
         uncond = uncond if isinstance(uncond, Cond) else Cond(uncond)
         with self._ctx():
             plan = self.plan(b, h, w)
-            plan.unet.set_context(torch.cat([cond.ctx, uncond.ctx]).to(self.dtype).contiguous())
+            plan.set_context(cond.ctx, uncond.ctx)
             # SDXL: the vector conditioning of [cond | uncond] enters through the time-embedding table (per-sample rows)
             self._y = None if cond.y is None else torch.cat([cond.y, uncond.y]).to(self.device)
             masked = inpaint is not None
@@ -732,7 +767,8 @@ class SDEngine:
     def img2img(self, tokens: torch.Tensor, neg_tokens: torch.Tensor, seed: int, init_u8: torch.Tensor,
                 denoising_strength: float = 0.75, steps: int = 20, cfg_scale: float = 7.0, sampler: str = "DDIM",
                 scheduler: Optional[str] = None, latmask: Optional[torch.Tensor] = None,
-                inpainting_fill: int = 1) -> torch.Tensor:
+                inpainting_fill: int = 1, multipliers: Optional[torch.Tensor] = None,
+                neg_multipliers: Optional[torch.Tensor] = None) -> torch.Tensor:
         """img2img: VAE-encode the init images (posterior mean), noise them to t_enc, run the remaining part of the
         sampler's schedule, decode.  init_u8 uint8 [b, H, W, 3].  Returns uint8 [b, H, W, 3] on device.
         `latmask` fp32 [h * w] (b200sd.inpaint.prepare_mask): inpainting — the region with latmask 0 is held to the init
@@ -743,7 +779,7 @@ class SDEngine:
         the request's start noise / by zeros first (sdwui Img2Img.init); 0 ("fill") is image-space work the caller does
         before the call (inpaint.fill_masked), 1 keeps the original content."""
         b = tokens.shape[0]
-        cond, uncond = self._conds(tokens, neg_tokens, init_u8.shape[2], init_u8.shape[1])
+        cond, uncond = self._conds(tokens, neg_tokens, init_u8.shape[2], init_u8.shape[1], multipliers, neg_multipliers)
         init = self.encode(init_u8)
         _, _, h, w = init.shape
         if latmask is not None and inpainting_fill in (2, 3):
@@ -770,7 +806,8 @@ class SDEngine:
     def txt2img_hires(self, tokens: torch.Tensor, neg_tokens: torch.Tensor, seed: int, steps: int = 20,
                       cfg_scale: float = 7.0, height: int = 512, width: int = 512, hr_scale: float = 2.0,
                       hr_steps: int = 0, denoising_strength: float = 0.7, sampler: str = "DDIM",
-                      scheduler: Optional[str] = None) -> torch.Tensor:
+                      scheduler: Optional[str] = None, multipliers: Optional[torch.Tensor] = None,
+                      neg_multipliers: Optional[torch.Tensor] = None) -> torch.Tensor:
         """txt2img with sdwui's hires fix and the "Latent" upscaler (StableDiffusionProcessingTxt2Img.sample /
         sample_hr_pass): first pass at (height, width), bilinear resize of the latents to hr_scale x, a fresh per-image
         noise of the large shape from the same seeds, then the same sampler's img2img half from t_enc with `hr_steps`
@@ -778,14 +815,14 @@ class SDEngine:
         b = tokens.shape[0]
         h, w = height // 8, width // 8
         h2, w2 = int(height * hr_scale) // 8, int(width * hr_scale) // 8
-        cond, uncond = self._conds(tokens, neg_tokens, width, height)
+        cond, uncond = self._conds(tokens, neg_tokens, width, height, multipliers, neg_multipliers)
         lat = self._sample_txt(cond, uncond, seed, b, h, w, steps, cfg_scale, sampler, scheduler)
         with self._ctx():
             up = torch.empty((b, h2 * w2, 4), device=self.device, dtype=torch.float32)
             ops.resize_latent_bilinear(lat.contiguous(), up, h, w, h2, w2)
         init = up.reshape(b, h2, w2, 4).permute(0, 3, 1, 2)
         if self.clip.xl:   # SDXL's vector conditioning carries the target size: the second pass gets its own (sdwui hr_c / hr_uc)
-            cond, uncond = self._conds(tokens, neg_tokens, w2 * 8, h2 * 8)
+            cond, uncond = self._conds(tokens, neg_tokens, w2 * 8, h2 * 8, multipliers, neg_multipliers)
         lat2 = self._sample_from(init, cond, uncond, seed, denoising_strength, hr_steps or steps, cfg_scale, sampler, scheduler)
         return self.decode(lat2, h2, w2)
 
@@ -797,10 +834,12 @@ class SDEngine:
 
     @torch.no_grad()
     def txt2img(self, tokens: torch.Tensor, neg_tokens: torch.Tensor, seed: int, steps: int = 20, cfg_scale: float = 7.0,
-                height: int = 512, width: int = 512, sampler: str = "DDIM", scheduler: Optional[str] = None) -> torch.Tensor:
-        """Whole request for this engine's share: returns uint8 [b, H, W, 3] on device."""
+                height: int = 512, width: int = 512, sampler: str = "DDIM", scheduler: Optional[str] = None,
+                multipliers: Optional[torch.Tensor] = None, neg_multipliers: Optional[torch.Tensor] = None) -> torch.Tensor:
+        """Whole request for this engine's share: returns uint8 [b, H, W, 3] on device.  tokens [b, 77 * k] and
+        neg_tokens [b, 77 * k'] with their optional emphasis multipliers of the same shapes (factory.tokenize_prompts)."""
         b = tokens.shape[0]
         h, w = height // 8, width // 8
-        cond, uncond = self._conds(tokens, neg_tokens, width, height)
+        cond, uncond = self._conds(tokens, neg_tokens, width, height, multipliers, neg_multipliers)
         lat = self._sample_txt(cond, uncond, seed, b, h, w, steps, cfg_scale, sampler, scheduler)
         return self.decode(lat, h, w)

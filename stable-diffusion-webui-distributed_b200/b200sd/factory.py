@@ -7,7 +7,7 @@ import logging
 import os
 import threading
 import zlib
-from typing import Dict, List
+from typing import Dict, List, Tuple
 
 import torch
 
@@ -106,7 +106,7 @@ def synthetic_tokens(prompts: List[str], vocab: int, ctx: int = 77) -> torch.Ten
     tok = _clip_tokenizer()
     if tok is not None:
         # the real BPE ids, padded with the end-of-text token like sdwui's FrozenCLIPEmbedderWithCustomWords (plain
-        # prompts up to 75 tokens; emphasis syntax, BREAK and >75-token chunking are not interpreted)
+        # prompts up to 75 tokens; emphasis syntax, BREAK and >75-token chunking are interpreted by tokenize_prompts)
         ids = tok(list(prompts), padding="max_length", max_length=ctx, truncation=True, return_tensors="pt").input_ids.long()
         eos = tok.eos_token_id
         first_eos = (ids == eos).float().argmax(dim=1)
@@ -116,6 +116,35 @@ def synthetic_tokens(prompts: List[str], vocab: int, ctx: int = 77) -> torch.Ten
             raise ValueError("the tokenizer's ids do not fit the text encoder's vocabulary")
         return ids
     return _hashed_tokens(prompts, vocab, ctx)
+
+
+def tokenize_prompts(prompts: List[str], vocab: int) -> Tuple[torch.Tensor, torch.Tensor]:
+    """Prompts with sdwui's syntax (b200sd.prompts: emphasis, BREAK, chunks of 75 tokens with comma backtracking) ->
+    (ids int64 [n, 77 * k], multipliers fp32 [n, 77 * k]); a prompt with fewer chunks than the longest one is padded with
+    empty chunks, as sdwui pads a batch.  Tokeniser: the CLIP BPE of SD_TOKENIZER (comma ",</w>"), otherwise the crc32
+    word hash of synthetic_tokens per segment (no comma token, so no backtracking).  A prompt without brackets, BREAK or
+    more than 75 tokens gets exactly synthetic_tokens' ids, all multipliers 1."""
+    from .prompts import tokenize_prompt
+    tok = _clip_tokenizer()
+    if tok is not None:
+        bos, eos = tok.bos_token_id, tok.eos_token_id
+        comma = tok.get_vocab().get(",</w>")
+
+        def ids_of(text):
+            return tok(text, truncation=False, add_special_tokens=False)["input_ids"] if text else []
+    else:
+        bos, eos, comma = vocab - 2, vocab - 1, None
+
+        def ids_of(text):
+            return [zlib.crc32(w.encode("utf-8")) % (vocab - 3) for w in text.split()]
+    per = [tokenize_prompt(p or "", ids_of, bos, eos, comma) for p in prompts]
+    k = max(len(c) for c, _ in per)
+    empty = [bos] + [eos] * 76
+    ids = torch.tensor([sum(c + [empty] * (k - len(c)), []) for c, _ in per], dtype=torch.long)
+    mult = torch.tensor([sum(m + [[1.0] * 77] * (k - len(m)), []) for _, m in per], dtype=torch.float32)
+    if int(ids.max()) >= vocab:
+        raise ValueError("the tokenizer's ids do not fit the text encoder's vocabulary")
+    return ids, mult
 
 
 def _hashed_tokens(prompts: List[str], vocab: int, ctx: int = 77) -> torch.Tensor:

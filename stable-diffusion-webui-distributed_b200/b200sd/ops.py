@@ -129,18 +129,30 @@ def conv2d(x: torch.Tensor, wt: torch.Tensor, out: torch.Tensor, ksize: int, str
 
 
 def attention(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, out: torch.Tensor, heads: int, d: int, d_pad: int,
-              scale: float, v_ones_col: bool = False):
+              scale: float, v_ones_col: bool = False, kv_len: Optional[torch.Tensor] = None):
     """q [B, Sq, >=heads*d_pad], k/v [B, Skv, >=heads*d_pad] (pitch = stride(1)), out [B, Sq, heads*d].
-    v_ones_col: v[..., h*d_pad + d] == 1 for every head (softmax denominators come out of the P.V MMA)."""
+    v_ones_col: v[..., h*d_pad + d] == 1 for every head (softmax denominators come out of the P.V MMA).
+    kv_len: int32 [B] on the device — row b attends to keys [0, kv_len[b]) only (b200sd_attention_varlen; the kernel
+    reads the lengths, so a captured graph follows later writes to the tensor).  None: every row attends to all Skv."""
     b, sq, _ = q.shape
     skv = k.shape[1]
     for t in (q, k, v, out):
         assert t.stride(2) == 1 and t.stride(0) == t.shape[1] * t.stride(1)
-    rc = _lib.lib().b200sd_attention(_p(q), ctypes.c_longlong(q.stride(1)), _p(k), ctypes.c_longlong(k.stride(1)),
-                                     _p(v), ctypes.c_longlong(v.stride(1)), _p(out), ctypes.c_longlong(out.stride(1)),
-                                     b, heads, sq, skv, d, d_pad, ctypes.c_float(scale), int(bool(v_ones_col)), _dt(q),
-                                     _stream())
-    check(rc, f"b200sd_attention B={b} h={heads} Sq={sq} Skv={skv} d={d}")
+    if kv_len is None:
+        rc = _lib.lib().b200sd_attention(_p(q), ctypes.c_longlong(q.stride(1)), _p(k), ctypes.c_longlong(k.stride(1)),
+                                         _p(v), ctypes.c_longlong(v.stride(1)), _p(out), ctypes.c_longlong(out.stride(1)),
+                                         b, heads, sq, skv, d, d_pad, ctypes.c_float(scale), int(bool(v_ones_col)),
+                                         _dt(q), _stream())
+        check(rc, f"b200sd_attention B={b} h={heads} Sq={sq} Skv={skv} d={d}")
+    else:
+        assert kv_len.dtype == torch.int32 and kv_len.is_contiguous() and kv_len.numel() == b
+        assert kv_len.device == q.device, "kv_len must live on the device"
+        rc = _lib.lib().b200sd_attention_varlen(_p(q), ctypes.c_longlong(q.stride(1)), _p(k),
+                                                ctypes.c_longlong(k.stride(1)), _p(v), ctypes.c_longlong(v.stride(1)),
+                                                _p(out), ctypes.c_longlong(out.stride(1)), b, heads, sq, skv,
+                                                _p(kv_len), d, d_pad, ctypes.c_float(scale), int(bool(v_ones_col)),
+                                                _dt(q), _stream())
+        check(rc, f"b200sd_attention_varlen B={b} h={heads} Sq={sq} Skv={skv} d={d}")
     _count()
     return out
 

@@ -9,7 +9,10 @@ from the reference at scripts/spartan/world.py:196 and, remotely, worker.py:432)
   * the timestep embedding depends only on t, never on x: `time_embed` + every ResBlock's `emb_layers` run ONCE
     per request for all sampler steps (as GEMM rows) and are folded into the conv1 biases; a tiny kernel selects
     the current step's bias rows on the device, so one captured graph replays for every step.
-  * cross-attention K/V of the (constant) text context are projected once per request.
+  * cross-attention K/V of the (constant) text context are projected once per request, into buffers of `ctx_len`
+    (the context capacity, a multiple of 77) rows per image.  A longer prompt grows them (grow_context); a grown
+    program attends row i to its own first kv_len[i] keys (b200sd_attention_varlen), so cond and uncond contexts of
+    different lengths share one batched evaluation and each gets what sdwui's separate UNet calls would give.
   * q/k/v projection weights carry zero rows so each head is padded to a multiple of 64 columns — exactly one
     TMA SWIZZLE_128B box per head chunk in the attention kernel.
 """
@@ -190,7 +193,11 @@ class UNetProgram:
         self.n, self.h, self.wd = n, h, wd
         self.dev, self.dt = w.device, w.dtype
         self.pool = Pool(self.dev, self.dt)
-        self.ctx_len = ctx_len
+        self.ctx_len = ctx_len      # context capacity: rows of every cross-attention K/V buffer
+        self.ctx_len0 = ctx_len     # ... as built: at this capacity the cross-attention calls take no lengths
+        # keys each batch row attends to, read by the kernels (graph replays follow it); used once the capacity grew
+        self.kv_len = torch.full((n,), ctx_len, device=self.dev, dtype=torch.int32)
+        self._xattn: List[tuple] = []   # (op index, transformer block, q, out, heads, d, d_pad, scale) per attn2
         cfg = self.cfg
         # persistent I/O
         self.xin = torch.zeros((n, h * wd, 64), device=self.dev, dtype=self.dt)    # latent channels 0..3, rest zero
@@ -212,13 +219,37 @@ class UNetProgram:
             holder[0] = self.stats_all
 
     # ---------------------------------------------------------------- per-request precompute
-    def set_context(self, ctx: torch.Tensor):
-        """ctx [N, ctx_len, context_dim] (cond rows first, uncond rows second): project K/V of every attn2 once."""
+    def set_context(self, ctx: torch.Tensor, lengths=None):
+        """ctx [N, L, context_dim] (cond rows first, uncond rows second), L <= ctx_len, rows of an image beyond its length
+        zero; lengths: tokens per row (None: L for every row).  Projects K/V of every attn2 once."""
         n, l, c = ctx.shape
-        assert n == self.n and l == self.ctx_len
+        assert n == self.n and l <= self.ctx_len, (ctx.shape, self.ctx_len)
+        lengths = [l] * n if lengths is None else [int(v) for v in lengths]
+        assert len(lengths) == n and all(1 <= v <= l for v in lengths), lengths
+        if self.ctx_len == self.ctx_len0:
+            assert all(v == self.ctx_len for v in lengths), "a context shorter than the capacity needs grow_context"
+        if l < self.ctx_len:   # zero rows up to the capacity: their keys are masked, their values finite
+            ctx = torch.cat([ctx, ctx.new_zeros((n, self.ctx_len - l, c))], dim=1)
+        l = self.ctx_len
         ctx2 = ctx.reshape(n * l, c)
         for key, buf in self.ctx_kv.items():
             ops.linear(ctx2, self.w.t[key + ".attn2.kv.w"], buf.reshape(n * l, -1), bias=self.w.t[key + ".attn2.kv.b"])
+        if self.ctx_len != self.ctx_len0:
+            self.kv_len.copy_(torch.tensor(lengths, dtype=torch.int32))
+
+    def grow_context(self, cap: int):
+        """Reallocate every cross-attention K/V buffer with `cap` rows per image (cap > ctx_len) and point the program's
+        attn2 launches at them, now with per-row key counts.  Activation buffers are untouched.  Graphs captured before
+        hold the old buffers' addresses: the caller drops them."""
+        assert cap > self.ctx_len
+        self.ctx_len = cap
+        for tb in list(self.ctx_kv):
+            old = self.ctx_kv[tb]
+            self.ctx_kv[tb] = torch.zeros((self.n, cap, old.shape[2]), device=self.dev, dtype=self.dt)
+        for i, tb, q2, o, heads, d, dp, scale in self._xattn:
+            kv = self.ctx_kv[tb]
+            self.ops[i] = (ops.attention, (q2, kv[..., :heads * dp], kv[..., heads * dp:], o, heads, d, dp, scale, dp > d),
+                           {"kv_len": self.kv_len})
 
     # ---------------------------------------------------------------- program construction
     def _emit(self, fn, *a, algo_flops=None, **k):
@@ -294,6 +325,7 @@ class UNetProgram:
             self._emit(ops.linear, a, t[tb + ".attn2.q.w"], q2, algo_flops=2.0 * n * hw * c * c)
             kv = torch.zeros((n, self.ctx_len, 2 * heads * dp), device=self.dev, dtype=self.dt)
             self.ctx_kv[tb] = kv
+            self._xattn.append((len(self.ops), tb, q2, o, heads, d, dp, scale))
             self._emit(ops.attention, q2, kv[..., :heads * dp], kv[..., heads * dp:], o, heads, d, dp, scale, dp > d)
             self.pool.put(q2)
             h2 = self.pool.get(n, hw, c)

@@ -143,7 +143,7 @@ class LocalGPUWorker(Worker):
             (isinstance(e, RuntimeError) and "CUDA" in str(e))
 
     def _generate(self, payload: dict) -> dict:
-        from b200sd.factory import synthetic_tokens
+        from b200sd.factory import tokenize_prompts
         eng = self.engine
         eng.interrupted = False
         batch = int(payload["batch_size"])
@@ -214,11 +214,15 @@ class LocalGPUWorker(Worker):
         cfg_scale = float(payload.get("cfg_scale", 7.0))
         strength = float(payload.get("subseed_strength") or 0.0)
         vocab = eng.clip_cfg.vocab
+        mult_all = None
         if "prompt_tokens" in payload:  # benchmark / tests hand pre-tokenised prompts through
             tok_all = torch.as_tensor(payload["prompt_tokens"]).long().reshape(-1, 77)
-        else:
-            tok_all = synthetic_tokens([prompt] * batch, vocab)
-        neg_all = synthetic_tokens([negative] * batch, vocab)
+        else:   # sdwui prompt syntax: emphasis weights, BREAK, 77-token chunks
+            tok_all, mult_all = tokenize_prompts([prompt] * batch, vocab)
+        neg_all, neg_mult = tokenize_prompts([negative] * batch, vocab)
+        # emphasis multipliers reach the engine only when some weight differs from 1 (all 1 is the unweighted path)
+        weighted = lambda m: m is not None and bool((m != 1.0).any())  # noqa: E731
+        weights = {"neg_multipliers": neg_mult} if weighted(neg_mult) else {}
         chunks = []
         for it in range(n_iter):
             # variation seeds: image k of iteration `it` blends noise(seed + k) with noise(subseed + k)
@@ -226,10 +230,12 @@ class LocalGPUWorker(Worker):
             eng.variation = (subseed + it * batch, strength) if strength != 0 else (None, 0.0)
             seed_it = seed if strength != 0 else seed + it * batch
             tok = tok_all[:batch] if tok_all.shape[0] >= batch else tok_all[:1].expand(batch, -1)
+            if weighted(mult_all):
+                weights["multipliers"] = mult_all[:batch]
             if init_u8 is not None:
                 kw = {} if inpaint is None else {"latmask": inpaint.latmask, "inpainting_fill": inpaint_fill}
                 u8 = eng.img2img(tok, neg_all, seed_it, init_u8, denoising_strength=denoise, steps=steps,
-                                 cfg_scale=cfg_scale, sampler=sampler, scheduler=scheduler, **kw)
+                                 cfg_scale=cfg_scale, sampler=sampler, scheduler=scheduler, **kw, **weights)
             elif payload.get("enable_hr"):
                 # hires fix (reference eta_hr, worker.py:205): second pass at hr_scale x with the "Latent" upscaler
                 upscaler = payload.get("hr_upscaler") or "Latent"
@@ -242,10 +248,10 @@ class LocalGPUWorker(Worker):
                                        width=width, hr_scale=hr_scale,
                                        hr_steps=int(payload.get("hr_second_pass_steps") or 0),
                                        denoising_strength=0.7 if ds is None else float(ds), sampler=sampler,
-                                       scheduler=scheduler)
+                                       scheduler=scheduler, **weights)
             else:
                 u8 = eng.txt2img(tok, neg_all, seed_it, steps=steps, cfg_scale=cfg_scale, height=height,
-                                 width=width, sampler=sampler, scheduler=scheduler)
+                                 width=width, sampler=sampler, scheduler=scheduler, **weights)
             chunks.append(u8)
             if eng.interrupted:
                 break
