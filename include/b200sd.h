@@ -5,8 +5,10 @@
  *   (`session.post(full_url("txt2img"|"img2img"))`, worker.py:432-435) whose process_images() runs
  *   UNet x steps + VAE decode.  The reference contains none of that arithmetic (SURVEY.md §0.2); these
  *   entry points are what a local executor binds instead of the HTTP call: every function below is one
- *   op of the per-step eps-prediction / final decode (SURVEY.md §8 a-ext x1..x11), taking raw device
- *   pointers and an explicit stream.
+ *   op of the per-step model evaluation and sampler update / final decode (SURVEY.md §8 a-ext x1..x11), taking
+ *   raw device pointers and an explicit stream.  The sampler updates take an eps-prediction model (SD1.x, SDXL);
+ *   the `_v` twins take a v-prediction model (SD 2.x 768-v and v-prediction finetunes): they convert the
+ *   CFG-combined v to eps = sqrt(1-a) x_in + sqrt(a) v in fp32, next to the fp32 latents, before the same update.
  *
  * Conventions
  *   - caller owns all device memory; the library never allocates, never synchronises, never throws
@@ -139,11 +141,27 @@ int b200sd_cfg_euler_a_step(const void* eps, long long pitch_e, float* x, const 
 int b200sd_cfg_dpmpp_2m_step(const void* eps, long long pitch_e, float* x, float* old_denoised, void* xin,
                              long long pitch_x, int B, int HW, float cfg_scale, const float* coef, int* step_counter,
                              int dtype, void* stream);
+/* v-prediction twins of the three fused steps: same arguments; `eps` holds the UNet's v output.  The CFG-combined v is
+ * converted with the kernel's own pre-update fp32 x (the point the UNet evaluated), then the eps step runs unchanged.
+ *   _ddim_step_v:     same 4-float rows; eps = sqrt(1-a_t) x + sqrt(a_t) v  (sdwui CompVisTimestepsVDenoiser)
+ *   _euler_a_step_v:  8-float rows {sigma, sigma_down, sigma_up, in_scale_next, kx, kv, 0, 0}
+ *   _dpmpp_2m_step_v: the 8-float rows with kx, kv in columns 5 and 6
+ * with kx = sigma/(sigma^2+1), kv = 1/sqrt(sigma^2+1): eps = kx x + kv v is to_d of k-diffusion's CompVisVDenoiser
+ * (sigma_data 1) on sigma-space x. */
+int b200sd_cfg_ddim_step_v(const void* eps, long long pitch_e, float* x, void* xin, long long pitch_x, int B, int HW,
+                           float cfg_scale, const float* coef, int* step_counter, int dtype, void* stream);
+int b200sd_cfg_euler_a_step_v(const void* eps, long long pitch_e, float* x, const float* noise, void* xin,
+                              long long pitch_x, int B, int HW, float cfg_scale, const float* coef, int* step_counter,
+                              int dtype, void* stream);
+int b200sd_cfg_dpmpp_2m_step_v(const void* eps, long long pitch_e, float* x, float* old_denoised, void* xin,
+                               long long pitch_x, int B, int HW, float cfg_scale, const float* coef, int* step_counter,
+                               int dtype, void* stream);
 /* ---- generic sampler building blocks: every sampler of the reference's ETA table (scripts/spartan/worker.py:75-94)
  * beyond the four fused ones above is, per model evaluation, one b200sd_cfg_eps plus a few b200sd_latent_lincomb on
  * fp32 NHWC latents [B,HW,4], with coefficient rows selected on the device by *step_counter (graph replay safe). */
 /* e = eps_uncond + cfg_scale * (eps_cond - eps_uncond), fp32 [B,HW,4].  (sdwui CFGDenoiser; equals k-diffusion
- * to_d(x, sigma, denoised) for the eps-prediction CompVisDenoiser) */
+ * to_d(x, sigma, denoised) for the eps-prediction CompVisDenoiser.  For a v-prediction model this is the CFG-combined v,
+ * and one b200sd_latent_lincomb e = kx x + kv e converts it to eps.) */
 int b200sd_cfg_eps(const void* eps, long long pitch_e, float* e, int B, int HW, float cfg_scale, int dtype, void* stream);
 /* dst = sum_{k<n_src} c[k] * srcs[k], c = coef + (*step_counter) * ld + col0.  srcs / idx_strides are HOST arrays of
  * n_src (<= 8) device pointers / element strides: a source with idx_strides[k] != 0 is a stack of tensors and tensor

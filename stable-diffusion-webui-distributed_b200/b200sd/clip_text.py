@@ -7,6 +7,8 @@ kernel scope ("run in torch").
   * SDXL (sgm GeneralConditioner, sd_xl_base.yaml): the CLIP-L tower read at hidden layer 11 (no final LN) next to an
     OpenCLIP ViT-bigG tower (penultimate layer; pooled = ln_final(last)[EOS] @ text_projection), and the vector
     conditioning cat(pooled, Fourier features of original size, crop, target size) that feeds the UNet's label_emb.
+  * SD 2.x (ldm FrozenOpenCLIPEmbedder, layer="penultimate"): the OpenCLIP ViT-H/14 tower run through all but its last
+    block, then ln_final.
   * Prompts longer than one chunk (sdwui FrozenCLIPEmbedderWithCustomWordsBase): tokens [B, 77 * k] are k separate
     77-token sequences through the tower, concatenated along the tokens; emphasis multipliers scale each chunk's output
     as sdwui's EmphasisOriginal does.
@@ -18,7 +20,7 @@ from typing import Dict, NamedTuple, Optional
 import torch
 import torch.nn.functional as F
 
-from .config import CLIP_PREFIX, XL_PREFIX0, XL_PREFIX1, CLIPConfig
+from .config import CLIP_PREFIX, OPENCLIP_PREFIX, XL_PREFIX0, XL_PREFIX1, CLIPConfig
 
 
 CAPTURE_LOCK = threading.Lock()   # CUDA graph captures are serialised across the per-device worker threads (engine.py too)
@@ -82,28 +84,23 @@ class ClipText:
 
 
 class OpenClipText:
-    """OpenCLIP text transformer (ViT-bigG-14 for SDXL): pre-LN resblocks with a packed in_proj, GELU MLP, causal mask"""
+    """OpenCLIP text transformer (ViT-bigG-14 for SDXL, ViT-H-14 for SD 2.x): pre-LN resblocks with a packed in_proj,
+    GELU MLP, causal mask.  Its size is the config's xl_* fields for SDXL's second tower, width / layers / heads for SD 2.x."""
 
     def __init__(self, sd: Dict[str, torch.Tensor], cfg: CLIPConfig, device, dtype, prefix: str = XL_PREFIX1):
         self.cfg, self.device, self.dtype = cfg, device, dtype
+        self.width, self.layers, self.heads = ((cfg.xl_width, cfg.xl_layers, cfg.xl_heads) if cfg.xl_width else
+                                               (cfg.width, cfg.layers, cfg.heads))
         n = len(prefix)
         self.w = {k[n:]: v.to(device=device, dtype=dtype) for k, v in sd.items() if k.startswith(prefix)}
 
-    @torch.no_grad()
-    def __call__(self, tokens: torch.Tensor):
-        """-> (penultimate residual stream [B, 77, W], pooled [B, proj])"""
-        w, cfg = self.w, self.cfg
-        tokens = tokens.to(self.device)
-        b, n = tokens.shape
-        wd, heads = cfg.xl_width, cfg.xl_heads
+    def _blocks(self, x: torch.Tensor, start: int, stop: int, mask: torch.Tensor) -> torch.Tensor:
+        """resblocks [start, stop) on the residual stream x [B, n, W]"""
+        w, wd, heads = self.w, self.width, self.heads
+        b, n, _ = x.shape
         d = wd // heads
-        x = w["token_embedding.weight"][tokens] + w["positional_embedding"][None, :n]
-        mask = torch.full((n, n), float("-inf"), device=self.device, dtype=torch.float32).triu(1)
-        penultimate = None
-        for i in range(cfg.xl_layers):
+        for i in range(start, stop):
             p = f"transformer.resblocks.{i}"
-            if i == cfg.xl_layers - 1:
-                penultimate = x
             h = F.layer_norm(x, (wd,), w[p + ".ln_1.weight"], w[p + ".ln_1.bias"], 1e-5)
             q, k, v = (t.reshape(b, n, heads, d).permute(0, 2, 1, 3)
                        for t in F.linear(h, w[p + ".attn.in_proj_weight"], w[p + ".attn.in_proj_bias"]).chunk(3, dim=-1))
@@ -112,9 +109,35 @@ class OpenClipText:
             h = F.layer_norm(x, (wd,), w[p + ".ln_2.weight"], w[p + ".ln_2.bias"], 1e-5)
             x = x + F.linear(F.gelu(F.linear(h, w[p + ".mlp.c_fc.weight"], w[p + ".mlp.c_fc.bias"])),
                              w[p + ".mlp.c_proj.weight"], w[p + ".mlp.c_proj.bias"])
+        return x
+
+    def _penultimate(self, tokens: torch.Tensor):
+        """(residual stream before the last resblock [B, n, W], causal mask)"""
+        w = self.w
+        n = tokens.shape[1]
+        x = w["token_embedding.weight"][tokens] + w["positional_embedding"][None, :n]
+        mask = torch.full((n, n), float("-inf"), device=self.device, dtype=torch.float32).triu(1)
+        return self._blocks(x, 0, self.layers - 1, mask), mask
+
+    @torch.no_grad()
+    def __call__(self, tokens: torch.Tensor):
+        """SDXL's second tower -> (penultimate residual stream [B, 77, W], pooled [B, proj])"""
+        w, wd = self.w, self.width
+        tokens = tokens.to(self.device)
+        b = tokens.shape[0]
+        penultimate, mask = self._penultimate(tokens)
+        x = self._blocks(penultimate, self.layers - 1, self.layers, mask)
         last = F.layer_norm(x, (wd,), w["ln_final.weight"], w["ln_final.bias"], 1e-5)
         pooled = last[torch.arange(b, device=self.device), tokens.argmax(dim=-1)] @ w["text_projection"]
         return penultimate, pooled
+
+    @torch.no_grad()
+    def encode(self, tokens: torch.Tensor) -> torch.Tensor:
+        """SD 2.x: tokens [B, 77] -> ln_final of the penultimate residual stream [B, 77, W] (ldm FrozenOpenCLIPEmbedder
+        with layer="penultimate": all but the last resblock run, then ln_final)"""
+        w, wd = self.w, self.width
+        x, _ = self._penultimate(tokens.to(self.device))
+        return F.layer_norm(x, (wd,), w["ln_final.weight"], w["ln_final.bias"], 1e-5)
 
 
 def fourier(scalars: torch.Tensor, dim: int) -> torch.Tensor:
@@ -138,6 +161,8 @@ class Conditioner:
         if self.xl:
             self.t0 = ClipText(sd, cfg, device, dtype, XL_PREFIX0)
             self.t1 = OpenClipText(sd, cfg, device, dtype, XL_PREFIX1)
+        elif cfg.open_clip:
+            self.t0 = OpenClipText(sd, cfg, device, dtype, OPENCLIP_PREFIX)
         else:
             self.t0 = ClipText(sd, cfg, device, dtype)
 
@@ -221,7 +246,8 @@ class Conditioner:
             return z.reshape(b, n, z.shape[-1])
 
         if not self.xl:
-            return Cond(ctx_of(self._chunked("t0", self.t0, seqs)[0]))
+            tower = self.t0.encode if self.cfg.open_clip else self.t0
+            return Cond(ctx_of(self._chunked("t0", tower, seqs)[0]))
         cfg = self.cfg
         (h0,) = self._chunked("t0_hidden", lambda t: self.t0.hidden(t, cfg.layers - 1), seqs)
         h1, pooled = self._chunked("t1", self.t1, seqs)

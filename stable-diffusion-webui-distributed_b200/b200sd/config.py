@@ -66,6 +66,12 @@ class CLIPConfig:
     xl_heads: int = 0
     xl_proj: int = 0          # text_projection output = pooled size (1280)
     size_embed_dim: int = 256  # ConcatTimestepEmbedderND outdim for the six size / crop scalars
+    # SD 2.x (ldm FrozenOpenCLIPEmbedder, layer="penultimate"): the single tower (width / layers / heads above) is an
+    # OpenCLIP text transformer under cond_stage_model.model., read as ln_final of the residual stream before its last block
+    open_clip: bool = False
+    # token after the first EOS of every 77-token chunk: None = EOS (CLIP); 0 for OpenCLIP (sdwui
+    # FrozenOpenCLIPEmbedderWithCustomWords: id_pad = 0)
+    pad_id: Optional[int] = None
 
     @property
     def context_dim(self) -> int:
@@ -90,12 +96,22 @@ TINYXL_UNET = UNetConfig(model_channels=64, channel_mult=(1, 2, 4), transformer_
 TINYXL_VAE = VAEConfig(ch=64, ch_mult=(1, 2), num_res_blocks=1, scale_factor=0.13025)
 TINYXL_CLIP = CLIPConfig(vocab=1000, width=64, layers=3, heads=2, xl_width=64, xl_layers=3, xl_heads=2, xl_proj=64,
                          size_embed_dim=32)
+# SD 2.x (v2-inference-v.yaml): d_head 64, Linear proj_in / proj_out, 1024-wide OpenCLIP ViT-H/14 context; SD1's VAE
+# (scale 0.18215) and noise schedule.  865 910 724 UNet parameters.  Served with v-prediction by default (768-v).
+SD21_UNET = UNetConfig(num_head_channels=64, context_dim=1024, linear_proj=True)
+SD21_VAE = VAEConfig()
+SD21_CLIP = CLIPConfig(width=1024, layers=24, heads=16, open_clip=True, pad_id=0)
+# SD 2.x topology at reduced width (d_head 64 in the UNet), for tests
+TINY21_UNET = UNetConfig(model_channels=64, num_head_channels=64, context_dim=64, linear_proj=True)
+TINY21_VAE = VAEConfig(ch=64, ch_mult=(1, 2), num_res_blocks=1)
+TINY21_CLIP = CLIPConfig(vocab=1000, width=64, layers=3, heads=2, open_clip=True, pad_id=0)
 XL_PREFIX0 = "conditioner.embedders.0.transformer.text_model."
 XL_PREFIX1 = "conditioner.embedders.1.model."
 
 UNET_PREFIX = "model.diffusion_model."
 VAE_PREFIX = "first_stage_model."
 CLIP_PREFIX = "cond_stage_model.transformer.text_model."
+OPENCLIP_PREFIX = "cond_stage_model.model."
 
 
 def unet_layout(cfg: UNetConfig):

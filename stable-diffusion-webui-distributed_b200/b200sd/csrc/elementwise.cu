@@ -159,7 +159,9 @@ __global__ void pack_unet_input_kernel(const float4* __restrict__ x, void* xin, 
   write_xin<kBf16>(xin, pitch, B, HW, i / HW, i % HW, v);
 }
 
-template <bool kBf16>
+// kVPred: the UNet predicts v (SD 2.x 768-v); the CFG-combined v becomes eps = sqrt(1-a_t) x + sqrt(a_t) v with the
+// pre-update fp32 x, the point the UNet evaluated (sdwui CompVisTimestepsVDenoiser.predict_eps_from_z_and_v)
+template <bool kBf16, bool kVPred = false>
 __global__ void cfg_ddim_step_kernel(const void* eps, long long pitch_e, float4* x, void* xin, long long pitch_x, int B,
                                      int HW, float cfg, const float* __restrict__ coef, int* step_counter) {
   pdl_trigger();
@@ -175,6 +177,10 @@ __global__ void cfg_ddim_step_kernel(const void* eps, long long pitch_e, float4*
     float e[4] = {eu.x + cfg * (ec.x - eu.x), eu.y + cfg * (ec.y - eu.y), eu.z + cfg * (ec.z - eu.z),
                   eu.w + cfg * (ec.w - eu.w)};
     float xs[4] = {xv.x, xv.y, xv.z, xv.w};
+    if constexpr (kVPred) {
+#pragma unroll
+      for (int k = 0; k < 4; ++k) e[k] = s1a * xs[k] + sa * e[k];
+    }
 #pragma unroll
     for (int k = 0; k < 4; ++k) {
       const float x0 = (xs[k] - s1a * e[k]) / sa;
@@ -188,15 +194,18 @@ __global__ void cfg_ddim_step_kernel(const void* eps, long long pitch_e, float4*
 
 // coef[step] = {sigma, sigma_down, sigma_up, in_scale_next}; x lives in sigma space (x = latent * sqrt(1+sigma^2));
 // the UNet input of the NEXT step is x_next * in_scale_next with in_scale_next = 1/sqrt(sigma_next^2 + 1).
-template <bool kBf16>
+// kVPred: rows of 8 floats {sigma, sigma_down, sigma_up, in_scale_next, kx, kv, 0, 0}; the CFG-combined v becomes
+// eps = kx x + kv v with kx = sigma/(sigma^2+1), kv = 1/sqrt(sigma^2+1) (k-diffusion CompVisVDenoiser: to_d of its denoised)
+template <bool kBf16, bool kVPred = false>
 __global__ void cfg_euler_a_step_kernel(const void* eps, long long pitch_e, float4* x, const float4* __restrict__ noise,
                                         void* xin, long long pitch_x, int B, int HW, float cfg,
                                         const float* __restrict__ coef, int* step_counter) {
   pdl_trigger();
   pdl_wait();
   const int step = *step_counter;
-  const float sigma = coef[step * 4 + 0], sdown = coef[step * 4 + 1], sup = coef[step * 4 + 2],
-              in_next = coef[step * 4 + 3];
+  constexpr int ld = kVPred ? 8 : 4;
+  const float sigma = coef[step * ld + 0], sdown = coef[step * ld + 1], sup = coef[step * ld + 2],
+              in_next = coef[step * ld + 3];
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i < B * HW) {
     const int b = i / HW, pix = i % HW;
@@ -206,6 +215,11 @@ __global__ void cfg_euler_a_step_kernel(const void* eps, long long pitch_e, floa
     float e[4] = {eu.x + cfg * (ec.x - eu.x), eu.y + cfg * (ec.y - eu.y), eu.z + cfg * (ec.z - eu.z),
                   eu.w + cfg * (ec.w - eu.w)};
     float xs[4] = {xv.x, xv.y, xv.z, xv.w};
+    if constexpr (kVPred) {
+      const float kx = coef[step * ld + 4], kv = coef[step * ld + 5];
+#pragma unroll
+      for (int k = 0; k < 4; ++k) e[k] = kx * xs[k] + kv * e[k];
+    }
     float nz[4] = {0.f, 0.f, 0.f, 0.f};
     if (noise != nullptr && sup > 0.f) {
       const float4 nv = noise[static_cast<long long>(step) * B * HW + i];
@@ -227,7 +241,8 @@ __global__ void cfg_euler_a_step_kernel(const void* eps, long long pitch_e, floa
 //   denoised = x - sigma * eps;  dd = c1 * denoised - c2 * old_denoised;  x = a * x + (1 - a) * dd;  old = denoised
 // with a = sigma_next / sigma = exp(-h), c1 = 1 + 1/(2r), c2 = 1/(2r), r = h_last / h (c1 = 1, c2 = 0 on the first step and
 // on the step to sigma = 0).  coef row = {sigma, a, c1, c2, in_scale_next, -, -, -}.
-template <bool kBf16>
+// kVPred: columns 5, 6 hold kx, kv and the CFG-combined v becomes eps = kx x + kv v (as in the Euler (a) kernel).
+template <bool kBf16, bool kVPred = false>
 __global__ void cfg_dpmpp_2m_step_kernel(const void* eps, long long pitch_e, float4* x, float4* old_denoised, void* xin,
                                          long long pitch_x, int B, int HW, float cfg, const float* __restrict__ coef,
                                          int* step_counter) {
@@ -242,9 +257,14 @@ __global__ void cfg_dpmpp_2m_step_kernel(const void* eps, long long pitch_e, flo
     const float4 ec = read_eps4<kBf16>(eps, pitch_e, static_cast<long long>(b) * HW + pix);
     const float4 eu = read_eps4<kBf16>(eps, pitch_e, static_cast<long long>(b + B) * HW + pix);
     const float4 xv = x[i], ov = old_denoised[i];
-    const float e[4] = {eu.x + cfg * (ec.x - eu.x), eu.y + cfg * (ec.y - eu.y), eu.z + cfg * (ec.z - eu.z),
-                        eu.w + cfg * (ec.w - eu.w)};
+    float e[4] = {eu.x + cfg * (ec.x - eu.x), eu.y + cfg * (ec.y - eu.y), eu.z + cfg * (ec.z - eu.z),
+                  eu.w + cfg * (ec.w - eu.w)};
     const float xs[4] = {xv.x, xv.y, xv.z, xv.w}, os[4] = {ov.x, ov.y, ov.z, ov.w};
+    if constexpr (kVPred) {
+      const float kx = coef[step * 8 + 5], kv = coef[step * 8 + 6];
+#pragma unroll
+      for (int k = 0; k < 4; ++k) e[k] = kx * xs[k] + kv * e[k];
+    }
     float xn[4], dn[4];
 #pragma unroll
     for (int k = 0; k < 4; ++k) {
@@ -461,49 +481,91 @@ extern "C" int b200sd_pack_unet_input(const float* x, void* xin, long long pitch
   RET_LAUNCH();
 }
 
-extern "C" int b200sd_cfg_ddim_step(const void* eps, long long pitch_e, float* x, void* xin, long long pitch_x, int B,
-                                    int HW, float cfg_scale, const float* coef, int* step_counter, int dtype,
-                                    void* stream) {
+template <bool kVPred>
+static int cfg_ddim_step(const void* eps, long long pitch_e, float* x, void* xin, long long pitch_x, int B, int HW,
+                         float cfg_scale, const float* coef, int* step_counter, int dtype, void* stream) {
   if (B <= 0) return B200SD_OK;
   if (pitch_e % 4 || pitch_x % 4) return B200SD_ERR_INVALID;
   const int n = B * HW;
   if (dtype == B200SD_BF16)
-    launch_pdl(cfg_ddim_step_kernel<true>, dim3((n + 255) / 256), dim3(256), 0, ST(stream), eps, pitch_e, reinterpret_cast<float4*>(x), xin, pitch_x, B, HW, cfg_scale, coef, step_counter);
+    launch_pdl(cfg_ddim_step_kernel<true, kVPred>, dim3((n + 255) / 256), dim3(256), 0, ST(stream), eps, pitch_e, reinterpret_cast<float4*>(x), xin, pitch_x, B, HW, cfg_scale, coef, step_counter);
   else
-    launch_pdl(cfg_ddim_step_kernel<false>, dim3((n + 255) / 256), dim3(256), 0, ST(stream), eps, pitch_e, reinterpret_cast<float4*>(x), xin, pitch_x, B, HW, cfg_scale, coef, step_counter);
+    launch_pdl(cfg_ddim_step_kernel<false, kVPred>, dim3((n + 255) / 256), dim3(256), 0, ST(stream), eps, pitch_e, reinterpret_cast<float4*>(x), xin, pitch_x, B, HW, cfg_scale, coef, step_counter);
   if (cudaGetLastError() != cudaSuccess) return B200SD_ERR_CUDA;
   launch_pdl(bump_step_kernel, dim3(1), dim3(1), 0, ST(stream), step_counter);
   RET_LAUNCH();
+}
+
+template <bool kVPred>
+static int cfg_euler_a_step(const void* eps, long long pitch_e, float* x, const float* noise, void* xin,
+                            long long pitch_x, int B, int HW, float cfg_scale, const float* coef, int* step_counter,
+                            int dtype, void* stream) {
+  if (B <= 0) return B200SD_OK;
+  if (pitch_e % 4 || pitch_x % 4) return B200SD_ERR_INVALID;
+  const int n = B * HW;
+  if (dtype == B200SD_BF16)
+    launch_pdl(cfg_euler_a_step_kernel<true, kVPred>, dim3((n + 255) / 256), dim3(256), 0, ST(stream), eps, pitch_e, reinterpret_cast<float4*>(x), reinterpret_cast<const float4*>(noise), xin, pitch_x, B, HW, cfg_scale, coef, step_counter);
+  else
+    launch_pdl(cfg_euler_a_step_kernel<false, kVPred>, dim3((n + 255) / 256), dim3(256), 0, ST(stream), eps, pitch_e, reinterpret_cast<float4*>(x), reinterpret_cast<const float4*>(noise), xin, pitch_x, B, HW, cfg_scale, coef, step_counter);
+  if (cudaGetLastError() != cudaSuccess) return B200SD_ERR_CUDA;
+  launch_pdl(bump_step_kernel, dim3(1), dim3(1), 0, ST(stream), step_counter);
+  RET_LAUNCH();
+}
+
+template <bool kVPred>
+static int cfg_dpmpp_2m_step(const void* eps, long long pitch_e, float* x, float* old_denoised, void* xin,
+                             long long pitch_x, int B, int HW, float cfg_scale, const float* coef, int* step_counter,
+                             int dtype, void* stream) {
+  if (B <= 0) return B200SD_OK;
+  if ((reinterpret_cast<uintptr_t>(x) | reinterpret_cast<uintptr_t>(old_denoised)) & 15) return B200SD_ERR_INVALID;
+  const int n = B * HW;
+  if (dtype == B200SD_BF16)
+    launch_pdl(cfg_dpmpp_2m_step_kernel<true, kVPred>, dim3((n + 255) / 256), dim3(256), 0, ST(stream), eps, pitch_e, reinterpret_cast<float4*>(x), reinterpret_cast<float4*>(old_denoised), xin, pitch_x, B, HW, cfg_scale, coef, step_counter);
+  else
+    launch_pdl(cfg_dpmpp_2m_step_kernel<false, kVPred>, dim3((n + 255) / 256), dim3(256), 0, ST(stream), eps, pitch_e, reinterpret_cast<float4*>(x), reinterpret_cast<float4*>(old_denoised), xin, pitch_x, B, HW, cfg_scale, coef, step_counter);
+  if (cudaGetLastError() != cudaSuccess) return B200SD_ERR_CUDA;
+  launch_pdl(bump_step_kernel, dim3(1), dim3(1), 0, ST(stream), step_counter);
+  RET_LAUNCH();
+}
+
+extern "C" int b200sd_cfg_ddim_step(const void* eps, long long pitch_e, float* x, void* xin, long long pitch_x, int B,
+                                    int HW, float cfg_scale, const float* coef, int* step_counter, int dtype,
+                                    void* stream) {
+  return cfg_ddim_step<false>(eps, pitch_e, x, xin, pitch_x, B, HW, cfg_scale, coef, step_counter, dtype, stream);
+}
+
+extern "C" int b200sd_cfg_ddim_step_v(const void* eps, long long pitch_e, float* x, void* xin, long long pitch_x, int B,
+                                      int HW, float cfg_scale, const float* coef, int* step_counter, int dtype,
+                                      void* stream) {
+  return cfg_ddim_step<true>(eps, pitch_e, x, xin, pitch_x, B, HW, cfg_scale, coef, step_counter, dtype, stream);
 }
 
 extern "C" int b200sd_cfg_euler_a_step(const void* eps, long long pitch_e, float* x, const float* noise, void* xin,
                                        long long pitch_x, int B, int HW, float cfg_scale, const float* coef,
                                        int* step_counter, int dtype, void* stream) {
-  if (B <= 0) return B200SD_OK;
-  if (pitch_e % 4 || pitch_x % 4) return B200SD_ERR_INVALID;
-  const int n = B * HW;
-  if (dtype == B200SD_BF16)
-    launch_pdl(cfg_euler_a_step_kernel<true>, dim3((n + 255) / 256), dim3(256), 0, ST(stream), eps, pitch_e, reinterpret_cast<float4*>(x), reinterpret_cast<const float4*>(noise), xin, pitch_x, B, HW, cfg_scale, coef, step_counter);
-  else
-    launch_pdl(cfg_euler_a_step_kernel<false>, dim3((n + 255) / 256), dim3(256), 0, ST(stream), eps, pitch_e, reinterpret_cast<float4*>(x), reinterpret_cast<const float4*>(noise), xin, pitch_x, B, HW, cfg_scale, coef, step_counter);
-  if (cudaGetLastError() != cudaSuccess) return B200SD_ERR_CUDA;
-  launch_pdl(bump_step_kernel, dim3(1), dim3(1), 0, ST(stream), step_counter);
-  RET_LAUNCH();
+  return cfg_euler_a_step<false>(eps, pitch_e, x, noise, xin, pitch_x, B, HW, cfg_scale, coef, step_counter, dtype,
+                                 stream);
+}
+
+extern "C" int b200sd_cfg_euler_a_step_v(const void* eps, long long pitch_e, float* x, const float* noise, void* xin,
+                                         long long pitch_x, int B, int HW, float cfg_scale, const float* coef,
+                                         int* step_counter, int dtype, void* stream) {
+  return cfg_euler_a_step<true>(eps, pitch_e, x, noise, xin, pitch_x, B, HW, cfg_scale, coef, step_counter, dtype,
+                                stream);
 }
 
 extern "C" int b200sd_cfg_dpmpp_2m_step(const void* eps, long long pitch_e, float* x, float* old_denoised, void* xin,
                                         long long pitch_x, int B, int HW, float cfg_scale, const float* coef,
                                         int* step_counter, int dtype, void* stream) {
-  if (B <= 0) return B200SD_OK;
-  if ((reinterpret_cast<uintptr_t>(x) | reinterpret_cast<uintptr_t>(old_denoised)) & 15) return B200SD_ERR_INVALID;
-  const int n = B * HW;
-  if (dtype == B200SD_BF16)
-    launch_pdl(cfg_dpmpp_2m_step_kernel<true>, dim3((n + 255) / 256), dim3(256), 0, ST(stream), eps, pitch_e, reinterpret_cast<float4*>(x), reinterpret_cast<float4*>(old_denoised), xin, pitch_x, B, HW, cfg_scale, coef, step_counter);
-  else
-    launch_pdl(cfg_dpmpp_2m_step_kernel<false>, dim3((n + 255) / 256), dim3(256), 0, ST(stream), eps, pitch_e, reinterpret_cast<float4*>(x), reinterpret_cast<float4*>(old_denoised), xin, pitch_x, B, HW, cfg_scale, coef, step_counter);
-  if (cudaGetLastError() != cudaSuccess) return B200SD_ERR_CUDA;
-  launch_pdl(bump_step_kernel, dim3(1), dim3(1), 0, ST(stream), step_counter);
-  RET_LAUNCH();
+  return cfg_dpmpp_2m_step<false>(eps, pitch_e, x, old_denoised, xin, pitch_x, B, HW, cfg_scale, coef, step_counter,
+                                  dtype, stream);
+}
+
+extern "C" int b200sd_cfg_dpmpp_2m_step_v(const void* eps, long long pitch_e, float* x, float* old_denoised, void* xin,
+                                          long long pitch_x, int B, int HW, float cfg_scale, const float* coef,
+                                          int* step_counter, int dtype, void* stream) {
+  return cfg_dpmpp_2m_step<true>(eps, pitch_e, x, old_denoised, xin, pitch_x, B, HW, cfg_scale, coef, step_counter,
+                                 dtype, stream);
 }
 
 

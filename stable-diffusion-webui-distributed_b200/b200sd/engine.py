@@ -24,6 +24,7 @@ MAX_PLANS = 6        # distinct (batch, latent h, w) kept per engine; the least 
 MAX_GRAPHS = 48      # step graphs kept per plan (one per sampler stage structure x cfg scale): oldest dropped beyond that
 CHUNK = 77           # tokens per prompt chunk (sdwui: [BOS] + 75 + [EOS]); contexts are 77 * k tokens long
 NOISE_SAMPLERS = ("Euler a", "stage")   # graph-name prefixes of the step graphs that may read Plan.noise
+PREDICTIONS = ("eps", "v")   # what the UNet predicts: the noise (SD1.x, SDXL, SD 2.x-base) or v (SD 2.x 768-v)
 # _CAPTURE_LOCK (imported): CUDA graph captures are serialised across the per-device worker threads
 
 
@@ -159,6 +160,20 @@ def dpmpp_2m_plan(steps: int, scheduler: str = "karras", sigmas=None):
     return t_out, rows, float(sig[0])
 
 
+def v_rows(fused: str, rows: List[List[float]]) -> List[List[float]]:
+    """coefficient rows of the fused k-diffusion steps for a v-prediction model: {kx, kv} of the row's sigma join them,
+    eps = kx x + kv v (CompVisVDenoiser, sigma_data 1).  Euler (a): 8-float rows {sigma, sigma_down, sigma_up, in_next,
+    kx, kv, 0, 0}; DPM++ 2M: columns 5, 6.  DDIM rows already hold sqrt(a_t), sqrt(1 - a_t)."""
+    if fused == "ddim":
+        return rows
+    out = []
+    for r in rows:
+        s = r[0]
+        kx, kv = s / (s * s + 1.0), 1.0 / math.sqrt(s * s + 1.0)
+        out.append(list(r[:4]) + [kx, kv, 0.0, 0.0] if fused in ("euler_a", "euler") else list(r[:5]) + [kx, kv, 0.0])
+    return out
+
+
 # sampler names of the sdwui API -> (method, scheduler).  sdwui >= 1.9 sends the scheduler separately ("scheduler" key,
 # "Automatic" = the sampler's default, which is Karras for DPM++ 2M); older versions fold it into the name.
 SAMPLERS = {"DDIM": ("ddim", None), "Euler a": ("euler_a", "uniform"), "Euler": ("euler", "uniform"),
@@ -269,6 +284,7 @@ class Plan:
         self.graphs: Dict[str, torch.cuda.CUDAGraph] = {}
         self.graph_launches: Dict[str, int] = {}
         self.stage_ids: Dict[tuple, int] = {}   # (lincomb structure, evaluated latent) of a generic stage -> graph-name id
+        self.vpred = eng.prediction == "v"      # the UNet output is v: the _v fused steps, one more lincomb per stage
 
     def noise_rows(self, rows: int) -> torch.Tensor:
         """the request's per-step noises live in ONE buffer per plan (the step graphs hold its raw address); it grows in
@@ -315,7 +331,10 @@ class Plan:
     def step_ddim(self, cfg_scale: float):
         ops.select_step(self.table, self.step, self.unet.cur_bias)
         self.unet.run()
-        ops.cfg_ddim_step(self.unet.eps, self.x, self.unet.xin, cfg_scale, self.coef, self.step)
+        if self.vpred:
+            ops.cfg_ddim_step_v(self.unet.eps, self.x, self.unet.xin, cfg_scale, self.coef, self.step)
+        else:
+            ops.cfg_ddim_step(self.unet.eps, self.x, self.unet.xin, cfg_scale, self.coef, self.step)
 
     def step_ddim_masked(self, cfg_scale: float):
         """inpainting (sdwui CFGDenoiserTimesteps, mask_before_denoising): the kept region of x is replaced by the clean
@@ -327,12 +346,18 @@ class Plan:
     def step_euler_a(self, cfg_scale: float):
         ops.select_step(self.table, self.step, self.unet.cur_bias)
         self.unet.run()
-        ops.cfg_euler_a_step(self.unet.eps, self.x, self.noise, self.unet.xin, cfg_scale, self.coef, self.step)
+        if self.vpred:
+            ops.cfg_euler_a_step_v(self.unet.eps, self.x, self.noise, self.unet.xin, cfg_scale, self.coef8, self.step)
+        else:
+            ops.cfg_euler_a_step(self.unet.eps, self.x, self.noise, self.unet.xin, cfg_scale, self.coef, self.step)
 
     def step_euler(self, cfg_scale: float):  # sigma_up == 0 in every coefficient row: the kernel needs no noise
         ops.select_step(self.table, self.step, self.unet.cur_bias)
         self.unet.run()
-        ops.cfg_euler_a_step(self.unet.eps, self.x, None, self.unet.xin, cfg_scale, self.coef, self.step)
+        if self.vpred:
+            ops.cfg_euler_a_step_v(self.unet.eps, self.x, None, self.unet.xin, cfg_scale, self.coef8, self.step)
+        else:
+            ops.cfg_euler_a_step(self.unet.eps, self.x, None, self.unet.xin, cfg_scale, self.coef, self.step)
 
     def stage(self, lcs, ev: str, cfg_scale: float, masked: bool, timestep_sampler: bool):
         """one model evaluation of a generic sampler program + its linear combinations (samplers.Stage.lcs)"""
@@ -343,6 +368,8 @@ class Plan:
         ops.select_step(self.table, self.step, self.unet.cur_bias)
         self.unet.run()
         ops.cfg_eps(self.unet.eps, lat["e"], cfg_scale)
+        if self.vpred:   # e holds the CFG-combined v: eps = kx ev + kv v, in fp32 next to the latents
+            ops.latent_lincomb(lat["e"], [lat[ev], lat["e"]], self.coefL, S.V_COL, self.step)
         if masked and not timestep_sampler:
             # k-diffusion samplers: denoised = denoised * nmask + init_latent * mask (CFGDenoiser.forward's last lines);
             # re-expressed on e = (ev - denoised) / sigma
@@ -359,7 +386,10 @@ class Plan:
     def step_dpmpp_2m(self, cfg_scale: float):
         ops.select_step(self.table, self.step, self.unet.cur_bias)
         self.unet.run()
-        ops.cfg_dpmpp_2m_step(self.unet.eps, self.x, self.old, self.unet.xin, cfg_scale, self.coef8, self.step)
+        if self.vpred:
+            ops.cfg_dpmpp_2m_step_v(self.unet.eps, self.x, self.old, self.unet.xin, cfg_scale, self.coef8, self.step)
+        else:
+            ops.cfg_dpmpp_2m_step(self.unet.eps, self.x, self.old, self.unet.xin, cfg_scale, self.coef8, self.step)
 
 
 class SDEngine:
@@ -369,7 +399,12 @@ class SDEngine:
         return torch.cuda.device(self.device) if self.device.type == "cuda" else contextlib.nullcontext()
 
     def __init__(self, sd: Dict[str, torch.Tensor], unet_cfg: UNetConfig, vae_cfg: VAEConfig, clip_cfg: CLIPConfig,
-                 device="cuda:0", dtype=torch.float16, use_graphs: bool = True, vae_chunk: int = 8):
+                 device="cuda:0", dtype=torch.float16, use_graphs: bool = True, vae_chunk: int = 8,
+                 prediction: str = "eps"):
+        """prediction: "eps" (the UNet predicts the noise) or "v" (v-parameterisation, SD 2.x 768-v and v finetunes)"""
+        if prediction not in PREDICTIONS:
+            raise ValueError(f"prediction {prediction!r} is not one of {PREDICTIONS}")
+        self.prediction = prediction
         self.device = torch.device(device)
         if self.device.type != "cuda" and self._require_cuda:
             raise RuntimeError("SDEngine needs a CUDA device: the hot path is sm_90a kernels only (no CPU fallback)")
@@ -524,6 +559,8 @@ class SDEngine:
             pr.fused = method
             fn = {"euler_a": euler_a_plan, "euler": euler_plan, "dpmpp_2m": dpmpp_2m_plan}[method]
             pr.ts, pr.rows, _ = fn(len(sig) - 1, sched, (sig, log_sig))
+            if self.prediction == "v":
+                pr.rows = v_rows(method, pr.rows)
             pr.draws = len(pr.rows) if method == "euler_a" else 0
             return pr
         sg = [float(v) for v in sig]
@@ -701,6 +738,8 @@ class SDEngine:
         if sigmas is not None:
             fn = {"euler_a": euler_a_plan, "euler": euler_plan, "dpmpp_2m": dpmpp_2m_plan}[pr.fused]
             pr.ts, pr.rows, sigma0 = fn(len(sigmas[0]) - 1, None, sigmas)
+            if self.prediction == "v":
+                pr.rows = v_rows(pr.fused, pr.rows)
             pr.noise_scale, pr.in0 = 1.0, S.c_in(sigma0)
             pr.draws = len(pr.rows) if pr.fused == "euler_a" else 0
         return self.run_program(cond, uncond, x_T.to(torch.float32) * pr.noise_scale, pr, cfg_scale, noises, inpaint)

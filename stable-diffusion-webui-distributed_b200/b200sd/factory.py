@@ -1,13 +1,15 @@
 """Engine construction for the local-GPU workers: one SDEngine per CUDA device, built lazily and cached.
 
-Weights: `SD_CKPT=/path/model.safetensors` (ldm key names) when present, otherwise the seeded synthetic SD1.5
-weights of synth.py (no checkpoint exists offline — every benchmark / parity number in this repo uses those).
+Weights: `SD_CKPT=/path/model.safetensors` (ldm key names; read for sd15 and sd21) when present, otherwise the seeded
+synthetic weights of synth.py (no checkpoint exists offline — every benchmark / parity number in this repo uses those).
+Model family: B200SD_MODEL = sd15 (default) | sdxl | sd21 | tiny | tinyxl | tiny21.  Prediction type: each family's
+default (v for sd21 / tiny21, eps for the others), overridden by B200SD_PREDICTION = eps | v.
 """
 import logging
 import os
 import threading
 import zlib
-from typing import Dict, List, Tuple
+from typing import Dict, List, Optional, Tuple
 
 import torch
 
@@ -19,6 +21,8 @@ log = logging.getLogger("distributed")
 _LOCK = threading.Lock()
 _ENGINES: Dict[str, SDEngine] = {}
 _STATE: Dict[str, Dict[str, torch.Tensor]] = {}
+CKPT_FAMILIES = ("sd15", "sd21")      # families whose weights SD_CKPT replaces (SDXL keeps its synthetic weights)
+V_FAMILIES = ("sd21", "tiny21")       # families served as v-prediction unless B200SD_PREDICTION says otherwise
 
 
 def _load_safetensors(path: str) -> Dict[str, torch.Tensor]:
@@ -31,7 +35,7 @@ def state_dict(size: str = "sd15", seed: int = 0) -> Dict[str, torch.Tensor]:
     with _LOCK:
         if key not in _STATE:
             ckpt = os.environ.get("SD_CKPT")
-            if ckpt and size == "sd15":
+            if ckpt and size in CKPT_FAMILIES:
                 _STATE[key] = _load_safetensors(ckpt)
             else:
                 cfgs = configs(size)
@@ -48,12 +52,28 @@ def configs(size: str = "sd15"):
         return C.SDXL_UNET, C.SDXL_VAE, C.SDXL_CLIP
     if size == "tinyxl":
         return C.TINYXL_UNET, C.TINYXL_VAE, C.TINYXL_CLIP
+    if size == "sd21":
+        return C.SD21_UNET, C.SD21_VAE, C.SD21_CLIP
+    if size == "tiny21":
+        return C.TINY21_UNET, C.TINY21_VAE, C.TINY21_CLIP
     raise ValueError(size)
+
+
+def prediction(size: str) -> str:
+    """what the family's UNet predicts: B200SD_PREDICTION (eps | v) when set, otherwise v for SD 2.x (768-v), eps for the
+    rest.  SD 2.x-base is B200SD_PREDICTION=eps; v-prediction SD1.5 / SDXL finetunes are B200SD_PREDICTION=v."""
+    env = os.environ.get("B200SD_PREDICTION", "").strip()
+    if env:
+        if env not in ("eps", "v"):
+            raise ValueError(f"B200SD_PREDICTION={env!r}: expected 'eps' or 'v'")
+        return env
+    return "v" if size in V_FAMILIES else "eps"
 
 
 def default_engine_factory(device: str, size: str = None) -> SDEngine:
     size = size or os.environ.get("B200SD_MODEL", "sd15")
-    key = f"{device}:{size}"
+    pred = prediction(size)
+    key = f"{device}:{size}:{pred}"
     with _LOCK:
         eng = _ENGINES.get(key)
     if eng is None:
@@ -64,7 +84,7 @@ def default_engine_factory(device: str, size: str = None) -> SDEngine:
             log.warning("b200sd: SD_TOKENIZER is not set — prompts are hashed to token ids, not BPE-tokenised")
         # SDXL runs in bf16 (BASELINE config 4; its VAE overflows fp16 — sdwui upcasts it, SURVEY App. C)
         dtype = torch.bfloat16 if size in ("sdxl", "tinyxl") else torch.float16
-        eng = SDEngine(state_dict(size), *configs(size), device=device, dtype=dtype)
+        eng = SDEngine(state_dict(size), *configs(size), device=device, dtype=dtype, prediction=pred)
         with _LOCK:
             _ENGINES[key] = eng
     return eng
@@ -84,7 +104,7 @@ def model_identity(size: str = None) -> str:
     """what /sd-models and /options report as the loaded checkpoint"""
     size = size or os.environ.get("B200SD_MODEL", "sd15")
     ckpt = os.environ.get("SD_CKPT")
-    return os.path.basename(ckpt) if ckpt and size == "sd15" else f"synthetic-{size}-seed0"
+    return os.path.basename(ckpt) if ckpt and size in CKPT_FAMILIES else f"synthetic-{size}-seed0"
 
 
 _TOKENIZER = {}
@@ -102,7 +122,8 @@ def _clip_tokenizer():
     return _TOKENIZER[path]
 
 
-def synthetic_tokens(prompts: List[str], vocab: int, ctx: int = 77) -> torch.Tensor:
+def synthetic_tokens(prompts: List[str], vocab: int, ctx: int = 77, pad: Optional[int] = None) -> torch.Tensor:
+    """pad: the id after the first EOS (None: EOS; SD 2.x's OpenCLIP tower: 0)"""
     tok = _clip_tokenizer()
     if tok is not None:
         # the real BPE ids, padded with the end-of-text token like sdwui's FrozenCLIPEmbedderWithCustomWords (plain
@@ -112,18 +133,21 @@ def synthetic_tokens(prompts: List[str], vocab: int, ctx: int = 77) -> torch.Ten
         first_eos = (ids == eos).float().argmax(dim=1)
         for i in range(ids.shape[0]):
             ids[i, int(first_eos[i]):] = eos
+            if pad is not None:
+                ids[i, int(first_eos[i]) + 1:] = pad
         if int(ids.max()) >= vocab:
             raise ValueError("the tokenizer's ids do not fit the text encoder's vocabulary")
         return ids
-    return _hashed_tokens(prompts, vocab, ctx)
+    return _hashed_tokens(prompts, vocab, ctx, pad)
 
 
-def tokenize_prompts(prompts: List[str], vocab: int) -> Tuple[torch.Tensor, torch.Tensor]:
+def tokenize_prompts(prompts: List[str], vocab: int, pad: Optional[int] = None) -> Tuple[torch.Tensor, torch.Tensor]:
     """Prompts with sdwui's syntax (b200sd.prompts: emphasis, BREAK, chunks of 75 tokens with comma backtracking) ->
     (ids int64 [n, 77 * k], multipliers fp32 [n, 77 * k]); a prompt with fewer chunks than the longest one is padded with
     empty chunks, as sdwui pads a batch.  Tokeniser: the CLIP BPE of SD_TOKENIZER (comma ",</w>"), otherwise the crc32
     word hash of synthetic_tokens per segment (no comma token, so no backtracking).  A prompt without brackets, BREAK or
-    more than 75 tokens gets exactly synthetic_tokens' ids, all multipliers 1."""
+    more than 75 tokens gets exactly synthetic_tokens' ids, all multipliers 1.  pad: the id after each chunk's first EOS
+    (None: EOS, CLIP; 0 for SD 2.x's OpenCLIP tower, whose tokenizer has the same vocabulary and merges)."""
     from .prompts import tokenize_prompt
     tok = _clip_tokenizer()
     if tok is not None:
@@ -137,9 +161,9 @@ def tokenize_prompts(prompts: List[str], vocab: int) -> Tuple[torch.Tensor, torc
 
         def ids_of(text):
             return [zlib.crc32(w.encode("utf-8")) % (vocab - 3) for w in text.split()]
-    per = [tokenize_prompt(p or "", ids_of, bos, eos, comma) for p in prompts]
+    per = [tokenize_prompt(p or "", ids_of, bos, eos, comma, pad) for p in prompts]
     k = max(len(c) for c, _ in per)
-    empty = [bos] + [eos] * 76
+    empty = [bos, eos] + [eos if pad is None else pad] * 75
     ids = torch.tensor([sum(c + [empty] * (k - len(c)), []) for c, _ in per], dtype=torch.long)
     mult = torch.tensor([sum(m + [[1.0] * 77] * (k - len(m)), []) for _, m in per], dtype=torch.float32)
     if int(ids.max()) >= vocab:
@@ -147,9 +171,10 @@ def tokenize_prompts(prompts: List[str], vocab: int) -> Tuple[torch.Tensor, torc
     return ids, mult
 
 
-def _hashed_tokens(prompts: List[str], vocab: int, ctx: int = 77) -> torch.Tensor:
+def _hashed_tokens(prompts: List[str], vocab: int, ctx: int = 77, pad: Optional[int] = None) -> torch.Tensor:
     """Deterministic stand-in for the CLIP BPE tokenizer (its vocabulary files are not available offline):
-    [BOS] + one id per whitespace-separated word (crc32 mod vocab-3) + [EOS] padding, length 77."""
+    [BOS] + one id per whitespace-separated word (crc32 mod vocab-3) + [EOS] padding, length 77 (with `pad`: one EOS,
+    then `pad`)."""
     bos, eos = vocab - 2, vocab - 1
     out = torch.full((len(prompts), ctx), eos, dtype=torch.long)
     out[:, 0] = bos
@@ -157,4 +182,6 @@ def _hashed_tokens(prompts: List[str], vocab: int, ctx: int = 77) -> torch.Tenso
         ids = [zlib.crc32(w.encode("utf-8")) % (vocab - 3) for w in (text or "").split()][: ctx - 2]
         if ids:
             out[i, 1:1 + len(ids)] = torch.tensor(ids)
+        if pad is not None:
+            out[i, 2 + len(ids):] = pad
     return out

@@ -294,6 +294,43 @@ def cfg_dpmpp_2m_step(eps: torch.Tensor, x: torch.Tensor, old_denoised: torch.Te
     _count(2)
 
 
+
+# v-prediction twins of the three fused steps (b200sd_cfg_*_step_v): `v` is the UNet output [2B, HW, pitch] of a
+# v-prediction model; the kernel converts the CFG-combined v to eps with its own pre-update fp32 x, then steps as above
+def cfg_ddim_step_v(v: torch.Tensor, x: torch.Tensor, xin: torch.Tensor, cfg_scale: float, coef: torch.Tensor,
+                    step_counter: torch.Tensor):
+    """coef [steps, 4]: the DDIM rows {sqrt(a_t), sqrt(1-a_t), sqrt(a_prev), sqrt(1-a_prev)}"""
+    b, hw, _ = x.shape
+    rc = _lib.lib().b200sd_cfg_ddim_step_v(_p(v), ctypes.c_longlong(v.stride(1)), _p(x), _p(xin),
+                                           ctypes.c_longlong(xin.stride(1)), b, hw, ctypes.c_float(cfg_scale), _p(coef),
+                                           _p(step_counter), _dt(xin), _stream())
+    check(rc, "b200sd_cfg_ddim_step_v")
+    _count(2)
+
+
+def cfg_euler_a_step_v(v: torch.Tensor, x: torch.Tensor, noise: Optional[torch.Tensor], xin: torch.Tensor,
+                       cfg_scale: float, coef8: torch.Tensor, step_counter: torch.Tensor):
+    """coef8 [steps, 8]: {sigma, sigma_down, sigma_up, in_scale_next, kx, kv, 0, 0}"""
+    b, hw, _ = x.shape
+    assert coef8.shape[-1] == 8
+    rc = _lib.lib().b200sd_cfg_euler_a_step_v(_p(v), ctypes.c_longlong(v.stride(1)), _p(x), _p(noise), _p(xin),
+                                              ctypes.c_longlong(xin.stride(1)), b, hw, ctypes.c_float(cfg_scale),
+                                              _p(coef8), _p(step_counter), _dt(xin), _stream())
+    check(rc, "b200sd_cfg_euler_a_step_v")
+    _count(2)
+
+
+def cfg_dpmpp_2m_step_v(v: torch.Tensor, x: torch.Tensor, old_denoised: torch.Tensor, xin: torch.Tensor,
+                        cfg_scale: float, coef8: torch.Tensor, step_counter: torch.Tensor):
+    """coef8 [steps, 8]: {sigma, sigma_next/sigma, c1, c2, in_scale_next, kx, kv, 0}"""
+    b, hw, _ = x.shape
+    assert coef8.shape[-1] == 8 and old_denoised.shape == x.shape
+    rc = _lib.lib().b200sd_cfg_dpmpp_2m_step_v(_p(v), ctypes.c_longlong(v.stride(1)), _p(x), _p(old_denoised), _p(xin),
+                                               ctypes.c_longlong(xin.stride(1)), b, hw, ctypes.c_float(cfg_scale),
+                                               _p(coef8), _p(step_counter), _dt(xin), _stream())
+    check(rc, "b200sd_cfg_dpmpp_2m_step_v")
+    _count(2)
+
 def image_to_nhwc(img_u8: torch.Tensor, out: torch.Tensor):
     """img_u8 uint8 [B, HW, 3] -> out [B, HW, pitch] channels 0..2 = 2*x/255 - 1"""
     b, hw, _ = img_u8.shape

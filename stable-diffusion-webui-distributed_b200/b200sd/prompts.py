@@ -6,7 +6,8 @@ What a remote sdwui does with `prompt` / `negative_prompt` before its text encod
     multiplies it by w; `\\(`, `\\)`, `\\[`, `\\]` and `\\\\` are literal characters; the word BREAK becomes a segment of
     its own with weight -1.
   * chunk_tokens: the segments' tokens are packed into chunks of 75 (FrozenCLIPEmbedderWithCustomWordsBase.tokenize_line),
-    each framed as [BOS] + tokens + [EOS] padding + [EOS], with one multiplier per token.
+    each framed as [BOS] + tokens + [EOS] padding + [EOS], with one multiplier per token.  A tower whose pad id is not EOS
+    (SD 2.x's OpenCLIP: 0) gets that id after the first EOS of every chunk (process_tokens).
 
 Not interpreted (as text they reach the tokenizer unchanged): prompt editing `[a:b:when]`, alternation `[a|b]`,
 composable `AND`, textual-inversion embeddings and extra-network tags.
@@ -76,11 +77,12 @@ def parse_prompt_attention(text: str) -> List[Tuple[str, float]]:
 
 
 def chunk_tokens(segments: Sequence[Tuple[Sequence[int], float, bool]], bos: int, eos: int,
-                 comma: Optional[int] = None, backtrack: int = COMMA_BACKTRACK) -> Tuple[List[List[int]], List[List[float]]]:
+                 comma: Optional[int] = None, backtrack: int = COMMA_BACKTRACK,
+                 pad: Optional[int] = None) -> Tuple[List[List[int]], List[List[float]]]:
     """[(token ids, weight, is_break)] -> (chunks of 77 ids, their 77 multipliers), sdwui's tokenize_line.
     A chunk takes 75 tokens.  When a full chunk is followed by a non-comma token and the chunk's last comma is within its
     last `backtrack` tokens, the tokens after that comma move to the next chunk.  BREAK closes the current chunk (an empty
-    one too).  An empty prompt is one chunk."""
+    one too).  An empty prompt is one chunk.  pad: the id after the first EOS of a chunk (None: EOS)."""
     chunks: List[List[int]] = []
     mults: List[List[float]] = []
     cur: List[int] = []
@@ -89,9 +91,9 @@ def chunk_tokens(segments: Sequence[Tuple[Sequence[int], float, bool]], bos: int
 
     def close(tokens, weights):
         nonlocal last_comma
-        pad = CHUNK_TOKENS - len(tokens)
-        chunks.append([bos] + tokens + [eos] * pad + [eos])
-        mults.append([1.0] + weights + [1.0] * pad + [1.0])
+        n_pad = CHUNK_TOKENS - len(tokens)
+        chunks.append([bos] + tokens + [eos] + [eos if pad is None else pad] * n_pad)
+        mults.append([1.0] + weights + [1.0] * n_pad + [1.0])
         last_comma = -1
 
     for ids, weight, is_break in segments:
@@ -119,8 +121,9 @@ def chunk_tokens(segments: Sequence[Tuple[Sequence[int], float, bool]], bos: int
 
 
 def tokenize_prompt(text: str, tokenize: Callable[[str], List[int]], bos: int, eos: int,
-                    comma: Optional[int] = None) -> Tuple[List[List[int]], List[List[float]]]:
-    """one prompt -> (chunks of 77 ids, multipliers); `tokenize` maps a segment's text to ids without BOS / EOS"""
+                    comma: Optional[int] = None, pad: Optional[int] = None) -> Tuple[List[List[int]], List[List[float]]]:
+    """one prompt -> (chunks of 77 ids, multipliers); `tokenize` maps a segment's text to ids without BOS / EOS; pad:
+    the id after each chunk's first EOS (None: EOS)"""
     segs = [((), w, True) if (t == "BREAK" and w == -1) else (tokenize(t), w, False)
             for t, w in parse_prompt_attention(text)]
-    return chunk_tokens(segs, bos, eos, comma)
+    return chunk_tokens(segs, bos, eos, comma, pad=pad)

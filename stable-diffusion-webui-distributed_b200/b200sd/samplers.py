@@ -8,6 +8,10 @@ depend on the step only.  The executor therefore needs two kernels beyond the UN
 `b200sd_latent_lincomb` (coefficient row selected on the device by the evaluation counter), and a stage's STRUCTURE (which
 tensors are combined into which) is a CUDA graph that replays for every evaluation with that structure.
 
+A v-prediction model (SD 2.x 768-v) changes one thing: the CFG-combined UNet output in `e` is v, and one more linear
+combination per evaluation, e = kx * ev + kv * e with the coefficients of the evaluated noise level (V_COL), turns it into
+the eps the stages below expect (k-diffusion CompVisVDenoiser / sdwui CompVisTimestepsVDenoiser, see Stage.row).
+
 This module is host arithmetic only (float64): it turns (sampler, sigma schedule | DDIM timesteps) into
     stages[i] = (structure, timestep for the time embedding, coefficient row)
 and says how many noise draws per image it needs and how they are mixed into the rows of the noise stack.
@@ -24,6 +28,7 @@ from typing import Callable, List, Sequence, Tuple
 COEF_LD = 32           # floats per coefficient row
 IDX_COL = COEF_LD - 1  # the row's last float = which tensor of the noise stack this stage reads
 MASK_COL = 24          # 4 floats {1, -sigma, 1/sigma, -1/sigma}: denoised = ev - sigma e and back (masked k-diffusion sampling)
+V_COL = 28             # 2 floats {kx, kv}: v-prediction models, eps = kx * ev + kv * v (Stage.row)
 
 # one linear combination: (dst, (src, ...), pack) — pack: the result, times one more coefficient, becomes the UNet input
 LC = Tuple[str, Tuple[str, ...], bool]
@@ -37,12 +42,18 @@ class Stage:
     ev: str = "x"                # which tensor the model was evaluated on (inpainting masks act on it / its denoised)
     sigma: float = 0.0           # its noise level (k-diffusion samplers; 0 for the timestep samplers)
     noise: int = -1              # row of the noise stack read by an 'n' source
+    alpha: float = 0.0           # alphas_cumprod at the evaluated timestep (timestep samplers; 0 for k-diffusion)
 
     def row(self) -> List[float]:
         assert len(self.coefs) <= MASK_COL, "coefficient row overflow"
         r = list(self.coefs) + [0.0] * (COEF_LD - len(self.coefs))
         if self.sigma > 0:
             r[MASK_COL:MASK_COL + 4] = [1.0, -self.sigma, 1.0 / self.sigma, -1.0 / self.sigma]
+            # v -> eps for sigma-space ev: ev * c_in is the UNet input and alphas_cumprod = 1 / (sigma^2 + 1)
+            r[V_COL:V_COL + 2] = [self.sigma / (self.sigma ** 2 + 1.0), 1.0 / math.sqrt(self.sigma ** 2 + 1.0)]
+        elif self.alpha > 0:
+            # v -> eps for latent-space ev (the UNet input itself): eps = sqrt(1 - a) ev + sqrt(a) v
+            r[V_COL:V_COL + 2] = [math.sqrt(1.0 - self.alpha), math.sqrt(self.alpha)]
         r[IDX_COL] = float(max(self.noise, 0))
         return r
 
@@ -295,12 +306,12 @@ def plms(ts: Sequence[int], ac: Sequence[float]) -> SamplerPlan:
         ce = math.sqrt(1 - ap) - math.sqrt(ap) * math.sqrt(1 - at) / math.sqrt(at)
         t_here, t_next = float(ts[index]), float(ts[max(index - 1, 0)])
         if n_old == 0:
-            st.append(Stage(MID_KEEP, t_here, [cx, ce, 1.0, 1.0], "x", 0.0))
-            st.append(Stage(FROM_H1, t_next, [cx, ce / 2, ce / 2, 1.0], "u", 0.0))
+            st.append(Stage(MID_KEEP, t_here, [cx, ce, 1.0, 1.0], "x", 0.0, alpha=at))
+            st.append(Stage(FROM_H1, t_next, [cx, ce / 2, ce / 2, 1.0], "u", 0.0, alpha=ap))   # ap = ac[t_next]
             n_old = 1
             continue
         w = {1: [3 / 2, -1 / 2, 0, 0], 2: [23 / 12, -16 / 12, 5 / 12, 0], 3: [55 / 24, -59 / 24, 37 / 24, -9 / 24]}[min(n_old, 3)]
-        st.append(Stage(MULTISTEP, t_here, [cx, *[ce * v for v in w], 1.0, 1.0, 1.0, 1.0], "x", 0.0))
+        st.append(Stage(MULTISTEP, t_here, [cx, *[ce * v for v in w], 1.0, 1.0, 1.0, 1.0], "x", 0.0, alpha=at))
         n_old += 1
     return SamplerPlan(st, 1.0, 1.0, timestep_sampler=True)
 

@@ -1,4 +1,4 @@
-"""Seeded synthetic weights with the exact SD1.5 parameter shapes and ldm state_dict key names.
+"""Seeded synthetic weights with the exact SD1.5 / SDXL / SD 2.x parameter shapes and state_dict key names.
 
 No checkpoint exists offline (SURVEY.md §8d): benchmarks, smoke and parity tests run on these.  Initialisation is
 variance preserving (N(0, 1/fan_in)) so 20 sampler steps stay numerically sane in fp16, and nothing is zero-initialised
@@ -9,8 +9,8 @@ from typing import Dict
 
 import torch
 
-from .config import (CLIP_PREFIX, UNET_PREFIX, VAE_PREFIX, XL_PREFIX0, XL_PREFIX1, CLIPConfig, UNetConfig, VAEConfig,
-                     unet_layout)
+from .config import (CLIP_PREFIX, OPENCLIP_PREFIX, UNET_PREFIX, VAE_PREFIX, XL_PREFIX0, XL_PREFIX1, CLIPConfig,
+                     UNetConfig, VAEConfig, unet_layout)
 
 
 class _Init:
@@ -157,11 +157,12 @@ def _vae(i: _Init, cfg: VAEConfig):
 
 
 def _open_clip(i: _Init, cfg: CLIPConfig, p: str):
-    """OpenCLIP text tower key names (sgm FrozenOpenCLIPEmbedder2.model)"""
-    w = cfg.xl_width
+    """OpenCLIP text tower key names (sgm FrozenOpenCLIPEmbedder2.model for SDXL's second tower; ldm
+    FrozenOpenCLIPEmbedder.model for SD 2.x, whose checkpoints also keep logit_scale)"""
+    w, layers, proj = (cfg.xl_width, cfg.xl_layers, cfg.xl_proj) if cfg.xl_width else (cfg.width, cfg.layers, cfg.width)
     i.sd[p + "token_embedding.weight"] = 0.02 * torch.randn((cfg.vocab, w), generator=i.g)
     i.sd[p + "positional_embedding"] = 0.01 * torch.randn((cfg.ctx, w), generator=i.g)
-    for l in range(cfg.xl_layers):
+    for l in range(layers):
         k = f"{p}transformer.resblocks.{l}"
         i.norm(k + ".ln_1", w)
         i.w(k + ".attn.in_proj_weight", (3 * w, w))
@@ -171,7 +172,9 @@ def _open_clip(i: _Init, cfg: CLIPConfig, p: str):
         i.lin(k + ".mlp.c_fc", 4 * w, w)
         i.lin(k + ".mlp.c_proj", w, 4 * w)
     i.norm(p + "ln_final", w)
-    i.sd[p + "text_projection"] = torch.randn((w, cfg.xl_proj), generator=i.g) / math.sqrt(w)
+    i.sd[p + "text_projection"] = torch.randn((w, proj), generator=i.g) / math.sqrt(w)
+    if not cfg.xl_width:
+        i.sd[p + "logit_scale"] = torch.tensor(math.log(1 / 0.07))
 
 
 def _clip(i: _Init, cfg: CLIPConfig, p: str = CLIP_PREFIX):
@@ -196,6 +199,8 @@ def make_state_dict(unet: UNetConfig, vae: VAEConfig, clip: CLIPConfig, seed: in
     if clip.xl_width:      # SDXL: sgm conditioner key names, two towers
         _clip(i, clip, XL_PREFIX0)
         _open_clip(i, clip, XL_PREFIX1)
+    elif getattr(clip, "open_clip", False):   # SD 2.x: one OpenCLIP tower (oracle configs lack the field)
+        _open_clip(i, clip, OPENCLIP_PREFIX)
     else:
         _clip(i, clip)
     return i.sd

@@ -214,12 +214,13 @@ class LocalGPUWorker(Worker):
         cfg_scale = float(payload.get("cfg_scale", 7.0))
         strength = float(payload.get("subseed_strength") or 0.0)
         vocab = eng.clip_cfg.vocab
+        pad = getattr(eng.clip_cfg, "pad_id", None)   # the token after each chunk's first EOS (SD 2.x: 0)
         mult_all = None
         if "prompt_tokens" in payload:  # benchmark / tests hand pre-tokenised prompts through
             tok_all = torch.as_tensor(payload["prompt_tokens"]).long().reshape(-1, 77)
         else:   # sdwui prompt syntax: emphasis weights, BREAK, 77-token chunks
-            tok_all, mult_all = tokenize_prompts([prompt] * batch, vocab)
-        neg_all, neg_mult = tokenize_prompts([negative] * batch, vocab)
+            tok_all, mult_all = tokenize_prompts([prompt] * batch, vocab, pad)
+        neg_all, neg_mult = tokenize_prompts([negative] * batch, vocab, pad)
         # emphasis multipliers reach the engine only when some weight differs from 1 (all 1 is the unweighted path)
         weighted = lambda m: m is not None and bool((m != 1.0).any())  # noqa: E731
         weights = {"neg_multipliers": neg_mult} if weighted(neg_mult) else {}
