@@ -76,7 +76,8 @@ int b200sd_attention(const void* Q, long long ldq, const void* K, long long ldk,
 /* b200sd_attention with a key count per batch row: row b attends to keys [0, kv_len[b]) of K/V buffers that are Skv
  * rows long.  kv_len is a DEVICE array of B ints, read by the kernel (one captured graph serves any lengths); each
  * length is clamped to [1, Skv].  Row b is bitwise equal to b200sd_attention on the first kv_len[b] key rows, provided
- * the buffer rows from kv_len[b] up to the next multiple of 64 (or Skv) hold finite values.  (sdwui evaluates a cond
+ * the buffer rows from kv_len[b] up to the next multiple of the key tile (128 when d <= 64, else 64) or Skv hold
+ * finite values.  (sdwui evaluates a cond
  * and an uncond context of different lengths in separate UNet calls; this evaluates them in one batch.) */
 int b200sd_attention_varlen(const void* Q, long long ldq, const void* K, long long ldk, const void* V, long long ldv,
                             void* O, long long ldo, int B, int heads, int Sq, int Skv, const int* kv_len, int d,

@@ -11,21 +11,29 @@
 // columns (never used: Q.K^T stops at d16, and P.V columns >= d are not stored) or, for the last head, the tensor map's
 // zero fill.  O is written unpadded ([b, s, h*d]) because it feeds the out-projection GEMM as a plain K-major A operand.
 //
-// One CTA = one 128-row Q tile of one (batch, head); 256 threads = two warpgroups, warpgroup w owns Q rows
-// [64w, 64w+64).  K / V are consumed in tiles of 64 rows through a ring of `stages` shared-memory slots that thread 0
-// refills by TMA (a slot is refilled once both warpgroups have released it).  Per kv tile and warpgroup:
-//   S = Q K^T        wgmma m64n64k16, A = Q and B = K both K-major in shared memory, S in registers
-//   online softmax   exact running maximum per row (the four threads of a row agree through two shuffles), P = 2^(S*scale*log2 e - m)
-//   O += P V         wgmma m64n(64*chunks)k16 with A = P from registers (the S accumulator fragment is the A fragment)
-//                    and B = V MN-major in shared memory
-// The row sums are accumulated in fp32 registers, so the ones column a caller may place in V (v_ones_col) is not needed
-// and its output column is not stored.
+// One CTA = one 128-row Q tile of one (batch, head); 384 threads, warp-specialised like the GEMM:
+//   * warpgroup 2 is the producer: one thread loads Q and runs the K / V ring (`stages` shared-memory slots of one kv
+//     tile each), refilling a slot once both math warpgroups have released it;
+//   * warpgroups 0 and 1 do the math, warpgroup w on Q rows [64w, 64w+64).
+// A kv tile is kKv = 128 rows for heads of one 64-column chunk (d <= 64) and 64 rows for two or three chunks, whose
+// wider O accumulator leaves no registers for a 128-wide S.  Per kv tile t and math warpgroup:
+//   S_t = Q K_t^T        wgmma m64n(kKv)k16, A = Q and B = K both K-major in shared memory, S in registers
+//   O += P_{t-1} V_{t-1} wgmma m64n(64*chunks)k16, A = P from registers (the S accumulator fragment is the A fragment),
+//                        B = V MN-major in shared memory; issued right behind S_t, so it runs during the softmax of S_t
+//   online softmax       exact running maximum of the raw logits per row (the four threads of a row agree through two
+//                        shuffles), P = 2^(S * c - m * c) with c = scale * log2 e, one FFMA and one MUFU.EX2 per element;
+//                        the columns >= Skv of a ragged last tile are masked (a separate instantiation of the loop body)
+//   O *= alpha           once P_{t-1} V_{t-1} has completed, outside any wgmma fence -> commit window
+// The two math warpgroups take turns at issuing their wgmma (named barriers 2 and 3), so the tensor core works for one
+// warpgroup while the other runs its softmax.  The row sums are accumulated in fp32 registers, so the ones column a
+// caller may place in V (v_ones_col) is not needed and its output column is not stored.  Rows >= Sq (zero-filled Q) are
+// computed like the others and only their stores are skipped, so both warpgroups always run the same number of turns.
 //
 // Varlen mode (b200sd_attention_varlen, kVarlen): batch row b attends to keys [0, kv_len[b]) of a K/V buffer that is Skv
 // rows long; kv_len is a device array, so one captured graph serves any split of lengths.  A CTA walks only the
-// ceil(kv_len[b] / 64) tiles it needs and masks columns >= kv_len[b] as the ragged tail of a plain call.  Tile walk and
+// ceil(kv_len[b] / kKv) tiles it needs and masks columns >= kv_len[b] as the ragged tail of a plain call.  Tile walk and
 // reduction order are those of a plain call with Skv = kv_len[b], so the results are bitwise equal to it as long as the
-// buffer rows in [kv_len[b], 64 * ceil(kv_len[b] / 64)) hold finite values (they get P = 0, where a plain call reads
+// buffer rows in [kv_len[b], kKv * ceil(kv_len[b] / kKv)) hold finite values (they get P = 0, where a plain call reads
 // the tensor map's zero fill).
 #include <cstddef>
 #include <cstdlib>
@@ -37,12 +45,12 @@
 
 namespace b200sd {
 
-constexpr int kAttnThreads = 256;                    // two warpgroups
+constexpr int kAttnMathThreads = 256;                       // two math warpgroups
+constexpr int kAttnThreads = kAttnMathThreads + 128;        // + the producer warpgroup
 constexpr int kQTile = 128;
-constexpr int kKv = 64;                              // kv rows per tile
 constexpr int kMaxStages = 3;
-constexpr uint32_t kQChunkBytes = kQTile * 128;      // 128 rows x 64 halfs
-constexpr uint32_t kKvChunkBytes = kKv * 128;        // 64 rows x 64 halfs
+constexpr uint32_t kQChunkBytes = kQTile * 128;             // 128 rows x 64 halfs
+__host__ __device__ constexpr int kv_tile(int chunks) { return chunks == 1 ? 128 : 64; }
 
 struct AttnParams {
   int B, heads, Sq, Skv, d, d_pad;
@@ -58,7 +66,7 @@ struct AttnParams {
 struct __align__(8) AttnShared {
   uint64_t q_full;
   uint64_t kv_full[kMaxStages];
-  uint64_t kv_empty[kMaxStages];  // one arrival per warpgroup
+  uint64_t kv_empty[kMaxStages];  // one arrival per math warpgroup
 };
 
 template <bool kBf16>
@@ -72,37 +80,103 @@ __device__ __forceinline__ uint32_t pack_h2(float a, float b) {
   }
 }
 
+// Ping-pong of the math warpgroups: warpgroup w issues its wgmma between turn_wait (bar.sync 2 + w) and turn_pass
+// (bar.arrive 3 - w, the other warpgroup's barrier).  Ids 2 and 3 stay clear of __syncthreads (0) and of the GEMM's
+// consumer barrier (1).
+__device__ __forceinline__ void turn_wait(int wg) {
+  asm volatile("bar.sync %0, %1;" ::"r"(2 + wg), "n"(kAttnMathThreads) : "memory");
+}
+__device__ __forceinline__ void turn_pass(int wg) {
+  asm volatile("bar.arrive %0, %1;" ::"r"(3 - wg), "n"(kAttnMathThreads) : "memory");
+}
+
+// Online softmax of one kv tile in place: s (the S accumulator, raw logits) becomes P = 2^(s * c - m * c) in fp32,
+// m_run / l_run advance, alpha = 2^((m_old - m_new) * c) is the factor O still has to be rescaled by.  kMask: columns
+// >= valid are -inf (the ragged last tile only).
+template <int kKv, bool kMask>
+__device__ __forceinline__ void softmax_tile(float (&s)[kKv / 2], float (&m_run)[2], float (&l_run)[2],
+                                             float (&alpha)[2], float c, int valid, int colq) {
+  float mx[2] = {-INFINITY, -INFINITY};
+#pragma unroll
+  for (int g = 0; g < kKv / 8; ++g)
+#pragma unroll
+    for (int h = 0; h < 2; ++h)
+#pragma unroll
+      for (int e = 0; e < 2; ++e) {
+        float& v = s[4 * g + 2 * h + e];
+        if constexpr (kMask) v = (8 * g + colq + e < valid) ? v : -INFINITY;
+        mx[h] = fmaxf(mx[h], v);
+      }
+  float mc[2];
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    mx[h] = fmaxf(mx[h], __shfl_xor_sync(0xffffffffu, mx[h], 1));
+    mx[h] = fmaxf(mx[h], __shfl_xor_sync(0xffffffffu, mx[h], 2));
+    const float m_new = fmaxf(m_run[h], mx[h]);     // finite: every kv tile has at least one valid column
+    alpha[h] = fast_exp2((m_run[h] - m_new) * c);  // 2^(-inf) = 0 on the first tile; exactly 1 while the max holds
+    m_run[h] = m_new;
+    mc[h] = m_new * c;
+    l_run[h] *= alpha[h];
+  }
+#pragma unroll
+  for (int g = 0; g < kKv / 8; ++g)
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      float& p0 = s[4 * g + 2 * h];
+      float& p1 = s[4 * g + 2 * h + 1];
+      p0 = fast_exp2(fmaf(p0, c, -mc[h]));
+      p1 = fast_exp2(fmaf(p1, c, -mc[h]));
+      l_run[h] += p0 + p1;
+    }
+}
+
+// S = Q K^T over kSteps k16 steps of the head dimension.  The count is a compile-time constant: ptxas serialises wgmma
+// issued from a run-time loop.
+// The descriptors of the later steps are those of step 0 plus the byte offset / 16 (start-address field, no carry: shared
+// memory ends below 256 KB).
+template <int kSteps, int kKv, bool kBf16>
+__device__ __forceinline__ void qk_tile(float (&s)[kKv / 2], uint64_t dq, uint64_t dk) {
+#pragma unroll
+  for (int ks = 0; ks < kSteps; ++ks) {
+    const uint32_t off = static_cast<uint32_t>(ks & 3) * 32u;  // k16 step inside the 128-byte swizzled row
+    Wgmma<kKv, kBf16>::ss(s, dq + ((static_cast<uint32_t>(ks >> 2) * kQChunkBytes + off) >> 4),
+                          dk + ((static_cast<uint32_t>(ks >> 2) * (kKv * 128u) + off) >> 4), ks != 0 ? 1u : 0u);
+  }
+}
+
 template <int kChunks, bool kBf16, bool kVarlen>
 __global__ void __launch_bounds__(kAttnThreads, 1)
 attention_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
                     const __grid_constant__ CUtensorMap tmV, const AttnParams p) {
-  constexpr int kDv = 64 * kChunks;  // MMA N of P.V
+  constexpr int kKv = kv_tile(kChunks);
+  constexpr int kDv = 64 * kChunks;                      // MMA N of P.V
+  // P_{t-1} V_{t-1} runs during the softmax of S_t; three chunks have no registers for S_t and P_{t-1} next to O
+  constexpr bool kOverlap = kChunks < 3;
+  constexpr uint32_t kKvChunkBytes = kKv * 128;          // kKv rows x 64 halfs
   constexpr uint32_t kKvBytes = kChunks * kKvChunkBytes;
   extern __shared__ uint8_t smem_raw[];
   pdl_trigger();  // pdl.cuh: the next kernel's prologue may overlap this kernel's tail
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint8_t* sQ = smem;                                   // chunks x (128 rows x 64)
-  uint8_t* sK = sQ + kChunks * kQChunkBytes;            // stages x chunks x (64 rows x 64)
+  uint8_t* sK = sQ + kChunks * kQChunkBytes;            // stages x chunks x (kKv rows x 64)
   uint8_t* sV = sK + p.stages * kKvBytes;
   AttnShared* sh = reinterpret_cast<AttnShared*>(sV + p.stages * kKvBytes);
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
-  const int wg = warp >> 2;
   const int qt = blockIdx.x;
   const int head = blockIdx.y;
   const int b = blockIdx.z;
   const int col0 = head * p.d_pad;
-  const bool loader = threadIdx.x == 0;
 
-  if (loader) {
+  if (threadIdx.x == kAttnMathThreads) {
     tma_prefetch_desc(&tmQ);
     tma_prefetch_desc(&tmK);
     tma_prefetch_desc(&tmV);
     mbar_init(&sh->q_full, 1);
     for (int s = 0; s < kMaxStages; ++s) {
       mbar_init(&sh->kv_full[s], 1);
-      mbar_init(&sh->kv_empty[s], 2);
+      mbar_init(&sh->kv_empty[s], kAttnMathThreads / 128);
     }
     fence_mbar_init();
   }
@@ -111,103 +185,122 @@ attention_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_consta
   const int skv = kVarlen ? min(max(p.kv_len[b], 1), p.Skv) : p.Skv;  // keys this batch row attends to
   const int nkv = (skv + kKv - 1) / kKv;
 
-  auto load_kv = [&](int t) {  // tile t into slot t % stages (the slot is free)
-    const int s = t % p.stages;
-    mbar_arrive_expect_tx(&sh->kv_full[s], 2 * kKvBytes);
+  if (warp >= kAttnMathThreads / 32) {
+    // ------------------------------- producer (one thread) -------------------------------
+    producer_warpgroup_regs();
+    if (threadIdx.x == kAttnMathThreads) {
+      mbar_arrive_expect_tx(&sh->q_full, kChunks * kQChunkBytes);
 #pragma unroll
-    for (int c = 0; c < kChunks; ++c) {
-      tma_load_3d(sK + s * kKvBytes + c * kKvChunkBytes, &tmK, &sh->kv_full[s], col0 + c * 64, t * kKv, b);
-      tma_load_3d(sV + s * kKvBytes + c * kKvChunkBytes, &tmV, &sh->kv_full[s], col0 + c * 64, t * kKv, b);
+      for (int c = 0; c < kChunks; ++c)
+        tma_load_3d(sQ + c * kQChunkBytes, &tmQ, &sh->q_full, col0 + c * 64, qt * kQTile, b);
+      for (int t = 0; t < nkv; ++t) {
+        const int s = t % p.stages;
+        // use u = t / stages of slot s: wait for the release of its use u - 1
+        if (t >= p.stages) mbar_wait(&sh->kv_empty[s], static_cast<uint32_t>(t / p.stages - 1) & 1u);
+        mbar_arrive_expect_tx(&sh->kv_full[s], 2 * kKvBytes);
+#pragma unroll
+        for (int c = 0; c < kChunks; ++c) {
+          tma_load_3d(sK + s * kKvBytes + c * kKvChunkBytes, &tmK, &sh->kv_full[s], col0 + c * 64, t * kKv, b);
+          tma_load_3d(sV + s * kKvBytes + c * kKvChunkBytes, &tmV, &sh->kv_full[s], col0 + c * 64, t * kKv, b);
+        }
+      }
     }
-  };
-  if (loader) {
-    mbar_arrive_expect_tx(&sh->q_full, kChunks * kQChunkBytes);
-#pragma unroll
-    for (int c = 0; c < kChunks; ++c) tma_load_3d(sQ + c * kQChunkBytes, &tmQ, &sh->q_full, col0 + c * 64, qt * kQTile, b);
-    for (int t = 0; t < p.stages && t < nkv; ++t) load_kv(t);
+    return;
   }
 
+  // ------------------------------- math warpgroups -------------------------------
+  consumer_warpgroup_regs();
+  const int wg = warp >> 2;
   const int colq = (lane & 3) * 2;  // accumulator columns 8g + colq, +1 of rows r0 (h = 0) and r0 + 8 (h = 1)
+  const bool signaller = (threadIdx.x & 127) == 0;  // releases ring slots for its warpgroup
+  const float c = p.scale_log2;
+  const bool ragged = skv % kKv != 0;
   const uint32_t sQ_a = smem_u32(sQ) + static_cast<uint32_t>(wg) * 8192u;
   const uint32_t sK_a = smem_u32(sK), sV_a = smem_u32(sV);
   float o[kDv / 2];
 #pragma unroll
   for (int i = 0; i < kDv / 2; ++i) o[i] = 0.f;
-  float m_run[2] = {-INFINITY, -INFINITY}, l_run[2] = {0.f, 0.f};
-  mbar_wait(&sh->q_full, 0);
+  float m_run[2] = {-INFINITY, -INFINITY}, l_run[2] = {0.f, 0.f}, alpha[2];
+  float sacc[kKv / 2];
+  uint32_t pa[kKv / 16][4];  // P of the previous tile as the A fragments of the k16 steps of P.V
 
-  for (int t = 0; t < nkv; ++t) {
-    // refill the slot of tile t-1 with tile t-1+stages once both warpgroups are done with it
-    if (loader && t > 0 && t - 1 + p.stages < nkv) {
-      const int s = (t - 1) % p.stages;
-      mbar_wait(&sh->kv_empty[s], static_cast<uint32_t>((t - 1) / p.stages) & 1u);
-      load_kv(t - 1 + p.stages);
-    }
-    const int s = t % p.stages;
-    mbar_wait(&sh->kv_full[s], static_cast<uint32_t>(t / p.stages) & 1u);
-
-    // S = Q K^T
-    float sacc[32];
-    const uint32_t k_a = sK_a + static_cast<uint32_t>(s) * kKvBytes;
-    wgmma_fence();
-    for (int ks = 0; ks < p.d16 / 16; ++ks) {
-      const uint32_t off = static_cast<uint32_t>(ks & 3) * 32u;  // k16 step inside the 128-byte swizzled row
-      Wgmma<64, kBf16>::ss(sacc, make_gdesc_sw128(sQ_a + static_cast<uint32_t>(ks >> 2) * kQChunkBytes + off, 16, 1024),
-                           make_gdesc_sw128(k_a + static_cast<uint32_t>(ks >> 2) * kKvChunkBytes + off, 16, 1024),
-                           ks != 0 ? 1u : 0u);
+  auto issue_qk = [&](int t) {  // S = Q K_t^T; d16 / 16 lies in [4 kChunks - 3, 4 kChunks]
+    const uint64_t dq = make_gdesc_sw128(sQ_a, 16, 1024);
+    const uint64_t dk = make_gdesc_sw128(sK_a + static_cast<uint32_t>(t % p.stages) * kKvBytes, 16, 1024);
+    switch (p.d16 / 16 - 4 * kChunks) {
+      case -3: qk_tile<4 * kChunks - 3, kKv, kBf16>(sacc, dq, dk); break;
+      case -2: qk_tile<4 * kChunks - 2, kKv, kBf16>(sacc, dq, dk); break;
+      case -1: qk_tile<4 * kChunks - 1, kKv, kBf16>(sacc, dq, dk); break;
+      default: qk_tile<4 * kChunks, kKv, kBf16>(sacc, dq, dk); break;
     }
     wgmma_commit();
-    wgmma_wait<0>();
-    reg_fence(sacc);
+  };
+  auto issue_pv = [&](int t) {  // O += P V_t
+    const uint64_t dv = make_gdesc_sw128(sV_a + static_cast<uint32_t>(t % p.stages) * kKvBytes, kKvChunkBytes, 1024);
+#pragma unroll
+    for (int j = 0; j < kKv / 16; ++j) Wgmma<kDv, kBf16>::rs_tb(o, pa[j], dv + static_cast<uint32_t>(j) * (2048u >> 4), 1u);
+    wgmma_commit();
+  };
+  auto softmax = [&](int t) {
+    if (ragged && t == nkv - 1) softmax_tile<kKv, true>(sacc, m_run, l_run, alpha, c, skv - t * kKv, colq);
+    else softmax_tile<kKv, false>(sacc, m_run, l_run, alpha, c, 0, colq);
+  };
+  auto pack_p = [&]() {
+#pragma unroll
+    for (int g = 0; g < kKv / 8; ++g)
+#pragma unroll
+      for (int h = 0; h < 2; ++h) pa[g >> 1][(g & 1) * 2 + h] = pack_h2<kBf16>(sacc[4 * g + 2 * h], sacc[4 * g + 2 * h + 1]);
+  };
 
-    // online softmax (scaled logits in log2 units); kv columns >= skv are masked
-    const int valid = skv - t * kKv;
-    float mx[2] = {-INFINITY, -INFINITY};
-#pragma unroll
-    for (int g = 0; g < 8; ++g)
-#pragma unroll
-      for (int h = 0; h < 2; ++h)
-#pragma unroll
-        for (int e = 0; e < 2; ++e) {
-          float& v = sacc[4 * g + 2 * h + e];
-          v = (8 * g + colq + e < valid) ? v * p.scale_log2 : -INFINITY;
-          mx[h] = fmaxf(mx[h], v);
-        }
-    float alpha[2];
-#pragma unroll
-    for (int h = 0; h < 2; ++h) {
-      mx[h] = fmaxf(mx[h], __shfl_xor_sync(0xffffffffu, mx[h], 1));
-      mx[h] = fmaxf(mx[h], __shfl_xor_sync(0xffffffffu, mx[h], 2));
-      const float m_new = fmaxf(m_run[h], mx[h]);  // finite: every kv tile has at least one valid column
-      alpha[h] = fast_exp2(m_run[h] - m_new);      // 2^(-inf) = 0 on the first tile
-      m_run[h] = m_new;
-      l_run[h] *= alpha[h];
+  // Turns: warpgroup 1 lets warpgroup 0 go first.  Each warpgroup takes nkv + 1 turns (S_0; S_t with P_{t-1} V_{t-1};
+  // the last P V) and passes after each; warpgroup 1 skips its last pass, which nobody waits for.
+  if (wg == 1) turn_pass(wg);
+  mbar_wait(&sh->q_full, 0);
+  mbar_wait(&sh->kv_full[0], 0);
+  turn_wait(wg);
+  wgmma_fence();
+  issue_qk(0);
+  turn_pass(wg);
+  wgmma_wait<0>();
+  reg_fence(sacc);
+  softmax(0);
+  pack_p();
+
+  for (int t = 1; t < nkv; ++t) {
+    mbar_wait(&sh->kv_full[t % p.stages], static_cast<uint32_t>(t / p.stages) & 1u);
+    turn_wait(wg);
+    reg_fence(o);
+    wgmma_fence();
+    if constexpr (kOverlap) {
+      issue_qk(t);
+      issue_pv(t - 1);
+    } else {
+      issue_pv(t - 1);
+      wgmma_wait<0>();  // P is dead: S_t may take its registers
+      reg_fence(o);
+      wgmma_fence();
+      issue_qk(t);
     }
+    turn_pass(wg);
+    wgmma_wait<kOverlap ? 1 : 0>();  // S_t has landed; with kOverlap, P_{t-1} V_{t-1} is still running
+    reg_fence(sacc);
+    softmax(t);
+    wgmma_wait<0>();
+    reg_fence(o);
+    if (signaller) mbar_arrive(&sh->kv_empty[(t - 1) % p.stages]);
 #pragma unroll
     for (int i = 0; i < kDv / 2; ++i) o[i] *= alpha[(i >> 1) & 1];
-    uint32_t pa[4][4];  // P as the A fragments of the four k16 steps of P.V
-#pragma unroll
-    for (int g = 0; g < 8; ++g)
-#pragma unroll
-      for (int h = 0; h < 2; ++h) {
-        const float p0 = fast_exp2(sacc[4 * g + 2 * h] - m_run[h]);
-        const float p1 = fast_exp2(sacc[4 * g + 2 * h + 1] - m_run[h]);
-        l_run[h] += p0 + p1;
-        pa[g >> 1][(g & 1) * 2 + h] = pack_h2<kBf16>(p0, p1);
-      }
-
-    // O += P V
-    const uint32_t v_a = sV_a + static_cast<uint32_t>(s) * kKvBytes;
-    reg_fence(o);
-    wgmma_fence();
-#pragma unroll
-    for (int j = 0; j < 4; ++j)
-      Wgmma<kDv, kBf16>::rs_tb(o, pa[j], make_gdesc_sw128(v_a + static_cast<uint32_t>(j) * 2048u, kKvChunkBytes, 1024), 1u);
-    wgmma_commit();
-    wgmma_wait<0>();
-    reg_fence(o);
-    if ((threadIdx.x & 127) == 0) mbar_arrive(&sh->kv_empty[s]);
+    pack_p();
   }
+
+  turn_wait(wg);
+  reg_fence(o);
+  wgmma_fence();
+  issue_pv(nkv - 1);
+  if (wg == 0) turn_pass(wg);
+  wgmma_wait<0>();
+  reg_fence(o);
+  if (signaller) mbar_arrive(&sh->kv_empty[(nkv - 1) % p.stages]);
 
   // O / l -> global (rows < Sq, columns < d)
 #pragma unroll
@@ -266,7 +359,7 @@ int attention_tc(const void* Q, long long ldq, const void* K, long long ldk, con
     return B200SD_ERR_INVALID;
   if (v_ones_col && d >= d_pad) return B200SD_ERR_INVALID;  // the ones column needs a free pad column
   if (kv_len && (reinterpret_cast<uintptr_t>(kv_len) & 3)) return B200SD_ERR_INVALID;
-  const int chunks = (d_pad + 63) / 64;
+  const int chunks = (((d + 15) & ~15) + 63) / 64;  // 64-column chunks that hold the d16 columns the MMAs read
   if (chunks > 3) return B200SD_ERR_UNSUPPORTED;
   {
     int dev = 0;
@@ -294,9 +387,10 @@ int attention_tc(const void* Q, long long ldq, const void* K, long long ldk, con
   p.scale_log2 = scale * 1.4426950408889634f;
   p.O = O; p.ldo = ldo;
   p.kv_len = kv_len;
-  const int nkv = (Skv + kKv - 1) / kKv;
+  const int kv = kv_tile(chunks);
+  const int nkv = (Skv + kv - 1) / kv;
   const size_t qt = static_cast<size_t>(chunks) * kQChunkBytes;
-  const size_t kvt = 2 * static_cast<size_t>(chunks) * kKvChunkBytes;  // K and V of one slot
+  const size_t kvt = 2 * static_cast<size_t>(chunks) * kv * 128;  // K and V of one slot
   p.stages = nkv < kMaxStages ? nkv : kMaxStages;
   const size_t smem = 1024 + qt + static_cast<size_t>(p.stages) * kvt + sizeof(AttnShared);
   if (smem > static_cast<size_t>(g_attn_max_smem)) return B200SD_ERR_UNSUPPORTED;
@@ -309,7 +403,7 @@ int attention_tc(const void* Q, long long ldq, const void* K, long long ldk, con
     const uint64_t st[2] = {static_cast<uint64_t>(ldq) * 2, static_cast<uint64_t>(ldq) * 2 * Sq};
     if ((rc = make_tmap_sw128(&tmQ, Q, 3, dims, st, box, es)) != B200SD_OK) return rc;
   }
-  const uint32_t kvbox[3] = {64, kKv, 1};
+  const uint32_t kvbox[3] = {64, static_cast<uint32_t>(kv), 1};
   {
     const uint64_t dims[3] = {static_cast<uint64_t>(heads) * d_pad, static_cast<uint64_t>(Skv), static_cast<uint64_t>(B)};
     const uint64_t st[2] = {static_cast<uint64_t>(ldk) * 2, static_cast<uint64_t>(ldk) * 2 * Skv};

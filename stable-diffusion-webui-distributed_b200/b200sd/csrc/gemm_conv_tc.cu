@@ -188,7 +188,7 @@ gemm_conv_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_consta
   if (warp >= kConsumerThreads / 32) {
     // ------------------------------- TMA producer (one thread) -------------------------------
     // The (tap, channel-block) position of the conv K loop is advanced by counters, not divisions.
-    setmaxnreg_dec<40>();
+    producer_warpgroup_regs();
     if (threadIdx.x == kConsumerThreads) {
       const int nkb = p.num_k_blocks, nstages = p.num_stages, cblocks = p.cblocks;
       const bool conv = p.mode == 1, taps9 = p.taps == 9;
@@ -230,7 +230,7 @@ gemm_conv_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_consta
   }
 
   // ------------------------------- consumer warpgroups -------------------------------
-  setmaxnreg_inc<232>();
+  consumer_warpgroup_regs();
   const int wg = warp >> 2;
   const int row0 = wg * 64 + (warp & 3) * 16 + (lane >> 2);  // this thread's accumulator rows: row0, row0 + 8
   const int colq = (lane & 3) * 2;                            // and columns 8g + colq, 8g + colq + 1

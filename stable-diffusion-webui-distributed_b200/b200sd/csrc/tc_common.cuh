@@ -121,6 +121,10 @@ template <int N>
 __device__ __forceinline__ void setmaxnreg_dec() {
   asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N) : "memory");
 }
+// Register split of the 384-thread warp-specialised kernels (two math warpgroups + one TMA producer warpgroup): the
+// producer keeps 40 registers per thread and the math warpgroups take 232 (2 x 128 x 232 + 128 x 40 <= 64 K).
+__device__ __forceinline__ void producer_warpgroup_regs() { setmaxnreg_dec<40>(); }
+__device__ __forceinline__ void consumer_warpgroup_regs() { setmaxnreg_inc<232>(); }
 // Keeps the compiler from moving reads / writes of an accumulator across a wgmma fence, commit or wait.
 template <int N>
 __device__ __forceinline__ void reg_fence(float (&d)[N]) {
