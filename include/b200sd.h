@@ -39,10 +39,13 @@ extern "C" {
 #define B200SD_EPI_GEGLU 1 /* tile columns [0,bn/2) = value, [bn/2,bn) = gate: out = v * gelu_erf(g) */
 #define B200SD_EPI_SILU 2  /* out = silu(acc + bias (+ residual)) */
 
+/* The residual may be the output itself (residual == D and ldr == ldd: D += epi(...) in place, e.g. a ControlNet zero
+ * conv adding into a channel slice of a skip-concat buffer): each output tile reads its residual tile before it
+ * stores that tile, and no two tiles overlap.  Any other overlap of residual and D is undefined. */
 typedef struct b200sd_epilogue {
   const float* bias;      /* [groups][N] fp32 or NULL */
   int bias_group_rows;    /* output rows sharing one bias row (H*W for a per-image bias); <=0: one row */
-  const void* residual;   /* [M][N_out] same dtype as the output, or NULL */
+  const void* residual;   /* [M][N_out] same dtype as the output, or NULL (may equal D, see above) */
   long long ldr;          /* residual row pitch (elements) */
   int flags;              /* B200SD_EPI_* */
 } b200sd_epilogue;
@@ -180,6 +183,10 @@ int b200sd_quantize_u8(const void* img, long long pitch, unsigned char* out, int
 /* img2img input: uint8 [B,HW,3] RGB -> [B,HW,pitch] with channel c < 3 = 2*x/255 - 1 (channels >= 3 untouched: zero
  * from allocation).  (sdwui StableDiffusionProcessingImg2Img.init) */
 int b200sd_image_to_nhwc(const unsigned char* img, void* out, long long pitch, int B, int HW, int dtype, void* stream);
+/* ControlNet hint: uint8 [B,HW,3] RGB -> [B,HW,pitch] with channel c < 3 = x/255 and channels 3..pitch-1 = 0 (ldm
+ * ControlNet input_hint_block input, sd-webui-controlnet's HWC3(image) / 255).  Not 2x/255 - 1: the hint block's zero
+ * padding at the image borders must stand for black. */
+int b200sd_hint_to_nhwc(const unsigned char* img, void* out, long long pitch, int B, int HW, int dtype, void* stream);
 /* VAE encoder moments [B,HW,pitch] (first 4 channels = posterior mean) -> scaled latents fp32 [B,HW,4] = mean * scale
  * (AutoencoderKL.encode(...).mean * scale_factor) */
 int b200sd_unpack_latent(const void* moments, long long pitch, float* x, int B, int HW, float scale, int dtype,

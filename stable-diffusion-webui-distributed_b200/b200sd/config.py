@@ -147,3 +147,23 @@ def unet_layout(cfg: UNetConfig):
                 layers.append(("up", ch))
             outputs.append(layers)
     return inputs, middle, outputs
+
+
+CONTROL_PREFIX = "control_model."
+# ldm ControlNet.input_hint_block: (cin, cout, stride) of its 8 convs 3x3, SiLU between them; the last one's cout is
+# model_channels
+HINT_CONVS = ((3, 16, 1), (16, 16, 1), (16, 32, 2), (32, 32, 1), (32, 96, 2), (96, 96, 1), (96, 256, 2))
+
+
+def controlnet_layout(cfg: UNetConfig):
+    """ldm ControlNet for a UNet of `cfg`: (input_blocks, middle_block, hint convs, zero-conv channels).  The encoder
+    and middle block are the UNet's own (unet_layout); hint convs are (cin, cout, stride) in state_dict order
+    input_hint_block.{0, 2, ..., 14}; zero conv i (1x1, zero_convs.i.0) follows input block i, middle_block_out.0 the
+    middle block."""
+    inputs, middle, _ = unet_layout(cfg)
+    hint = HINT_CONVS + ((256, cfg.model_channels, 1),)
+    zero_ch = []
+    for layers in inputs:
+        last = layers[0]
+        zero_ch.append(last[2] if last[0] in ("conv_in", "res") else last[1])
+    return inputs, middle, hint, zero_ch

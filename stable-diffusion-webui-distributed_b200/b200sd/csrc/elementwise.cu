@@ -361,6 +361,16 @@ __global__ void image_to_nhwc_kernel(const unsigned char* __restrict__ img, void
   for (int c = 0; c < 3; ++c) store1<kBf16>(out, i * pitch + c, static_cast<float>(img[i * 3 + c]) * (2.0f / 255.0f) - 1.0f);
 }
 
+// ControlNet hint: x / 255 (IEEE division, as torch computes it) in channels 0..2, zero in the rest of the row, so the
+// hint block's first conv sees exact zeros both in its padded channels and at the image borders
+template <bool kBf16>
+__global__ void hint_to_nhwc_kernel(const unsigned char* __restrict__ img, void* out, long long pitch, long long npix) {
+  const long long i = blockIdx.x * static_cast<long long>(blockDim.y) + threadIdx.y;   // one pixel per warp row
+  if (i >= npix) return;
+  for (long long c = threadIdx.x; c < pitch; c += blockDim.x)
+    store1<kBf16>(out, i * pitch + c, c < 3 ? static_cast<float>(img[i * 3 + c]) / 255.0f : 0.0f);
+}
+
 template <bool kBf16>
 __global__ void unpack_latent_kernel(const void* m, long long pitch, float4* x, long long npix, float scale) {
   const long long i = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x;
@@ -616,6 +626,18 @@ extern "C" int b200sd_image_to_nhwc(const unsigned char* img, void* out, long lo
   const int blocks = static_cast<int>((n + 255) / 256);
   if (dtype == B200SD_BF16) image_to_nhwc_kernel<true><<<blocks, 256, 0, ST(stream)>>>(img, out, pitch, n);
   else image_to_nhwc_kernel<false><<<blocks, 256, 0, ST(stream)>>>(img, out, pitch, n);
+  RET_LAUNCH();
+}
+
+extern "C" int b200sd_hint_to_nhwc(const unsigned char* img, void* out, long long pitch, int B, int HW, int dtype,
+                                   void* stream) {
+  if (B <= 0 || HW <= 0) return B200SD_OK;
+  if (pitch < 3) return B200SD_ERR_INVALID;
+  const long long n = static_cast<long long>(B) * HW;
+  const dim3 block(32, 8);
+  const int blocks = static_cast<int>((n + 7) / 8);
+  if (dtype == B200SD_BF16) hint_to_nhwc_kernel<true><<<blocks, block, 0, ST(stream)>>>(img, out, pitch, n);
+  else hint_to_nhwc_kernel<false><<<blocks, block, 0, ST(stream)>>>(img, out, pitch, n);
   RET_LAUNCH();
 }
 

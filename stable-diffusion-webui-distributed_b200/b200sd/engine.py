@@ -16,7 +16,7 @@ from . import ops
 from . import samplers as S
 from .clip_text import CAPTURE_LOCK as _CAPTURE_LOCK, Cond, Conditioner
 from .config import CLIPConfig, UNetConfig, VAEConfig
-from .unet_exec import TimeEmbedding, UNetProgram, UNetWeights
+from .unet_exec import MAX_CONTROLS, ControlNetWeights, TimeEmbedding, UNetProgram, UNetWeights
 from .vae_exec import VAEDecoderProgram, VAEDecoderWeights, VAEEncoderProgram, VAEEncoderWeights
 
 MAX_STEPS = 256
@@ -246,6 +246,7 @@ class Program:
     noise_scale: float = 1.0
     in0: float = 1.0                     # scale of the first UNet input
     timestep_sampler: bool = False
+    steps: int = 0                       # sampler steps requested (DPM adaptive: the n of ControlNet windows)
 
     def start(self, noise0: torch.Tensor, init: Optional[torch.Tensor] = None) -> torch.Tensor:
         x = noise0 * self.noise_scale
@@ -327,46 +328,53 @@ class Plan:
         ctx[b:, :lu] = uncond_ctx
         self.unet.set_context(ctx, [lc] * b + [lu] * b)
 
+    def _unet(self, active):
+        """one UNet evaluation with the ControlNet slots `active`; without any, the same call as ever"""
+        if active:
+            self.unet.run(active)
+        else:
+            self.unet.run()
+
     # one sampler step = select this step's biases, UNet on [cond | uncond], CFG + update + repack
-    def step_ddim(self, cfg_scale: float):
+    def step_ddim(self, cfg_scale: float, active=()):
         ops.select_step(self.table, self.step, self.unet.cur_bias)
-        self.unet.run()
+        self._unet(active)
         if self.vpred:
             ops.cfg_ddim_step_v(self.unet.eps, self.x, self.unet.xin, cfg_scale, self.coef, self.step)
         else:
             ops.cfg_ddim_step(self.unet.eps, self.x, self.unet.xin, cfg_scale, self.coef, self.step)
 
-    def step_ddim_masked(self, cfg_scale: float):
+    def step_ddim_masked(self, cfg_scale: float, active=()):
         """inpainting (sdwui CFGDenoiserTimesteps, mask_before_denoising): the kept region of x is replaced by the clean
         init latent before every model call"""
         ops.blend_latent(self.x, self.init, self.latmask)
         ops.pack_unet_input(self.x, self.unet.xin, 1.0)
-        self.step_ddim(cfg_scale)
+        self.step_ddim(cfg_scale, active)
 
-    def step_euler_a(self, cfg_scale: float):
+    def step_euler_a(self, cfg_scale: float, active=()):
         ops.select_step(self.table, self.step, self.unet.cur_bias)
-        self.unet.run()
+        self._unet(active)
         if self.vpred:
             ops.cfg_euler_a_step_v(self.unet.eps, self.x, self.noise, self.unet.xin, cfg_scale, self.coef8, self.step)
         else:
             ops.cfg_euler_a_step(self.unet.eps, self.x, self.noise, self.unet.xin, cfg_scale, self.coef, self.step)
 
-    def step_euler(self, cfg_scale: float):  # sigma_up == 0 in every coefficient row: the kernel needs no noise
+    def step_euler(self, cfg_scale: float, active=()):  # sigma_up == 0 in every coefficient row: the kernel needs no noise
         ops.select_step(self.table, self.step, self.unet.cur_bias)
-        self.unet.run()
+        self._unet(active)
         if self.vpred:
             ops.cfg_euler_a_step_v(self.unet.eps, self.x, None, self.unet.xin, cfg_scale, self.coef8, self.step)
         else:
             ops.cfg_euler_a_step(self.unet.eps, self.x, None, self.unet.xin, cfg_scale, self.coef, self.step)
 
-    def stage(self, lcs, ev: str, cfg_scale: float, masked: bool, timestep_sampler: bool):
+    def stage(self, lcs, ev: str, cfg_scale: float, masked: bool, timestep_sampler: bool, active=()):
         """one model evaluation of a generic sampler program + its linear combinations (samplers.Stage.lcs)"""
         lat = self.lat
         if masked and timestep_sampler:   # sdwui CFGDenoiser, mask_before_denoising: the evaluated tensor is blended first
             ops.blend_latent(lat[ev], self.init, self.latmask)
             ops.pack_unet_input(lat[ev], self.unet.xin, 1.0)
         ops.select_step(self.table, self.step, self.unet.cur_bias)
-        self.unet.run()
+        self._unet(active)
         ops.cfg_eps(self.unet.eps, lat["e"], cfg_scale)
         if self.vpred:   # e holds the CFG-combined v: eps = kx ev + kv v, in fp32 next to the latents
             ops.latent_lincomb(lat["e"], [lat[ev], lat["e"]], self.coefL, S.V_COL, self.step)
@@ -383,9 +391,9 @@ class Plan:
             col += len(srcs) + int(pack)
         ops.bump_step(self.step)
 
-    def step_dpmpp_2m(self, cfg_scale: float):
+    def step_dpmpp_2m(self, cfg_scale: float, active=()):
         ops.select_step(self.table, self.step, self.unet.cur_bias)
-        self.unet.run()
+        self._unet(active)
         if self.vpred:
             ops.cfg_dpmpp_2m_step_v(self.unet.eps, self.x, self.old, self.unet.xin, cfg_scale, self.coef8, self.step)
         else:
@@ -423,6 +431,7 @@ class SDEngine:
         self.interrupted = False
         self.variation = (None, 0.0)   # (subseed, subseed_strength) of the request being served: sdwui variation seeds
         self._y = None                 # SDXL vector conditioning of the run in progress
+        self._windows = []             # (guidance_start, guidance_end) of the run's ControlNet unit in each slot
         self._cap_stream = None
         self.last_unet_evals = 0
         self.graph_replayed_launches = 0   # b200sd kernels launched through graph replays (bench.py gpu_launches)
@@ -524,7 +533,7 @@ class SDEngine:
         reference's table.  With `denoise` the program is the img2img half: the sampler's schedule from t_enc on
         (sdwui sd_samplers_timesteps.sample_img2img / KDiffusionSampler.sample_img2img)."""
         method, sched = resolve_sampler(sampler, scheduler)
-        pr = Program(sampler, method)
+        pr = Program(sampler, method, steps=steps)
         if method in ("ddim", "plms"):
             ac = alphas_cumprod().double()
             ts_all = torch.clamp(torch.arange(0, 1000, 1000 // steps) + 1, 0, 999)
@@ -579,19 +588,56 @@ class SDEngine:
         pr.draws = pr.sp.draws
         return pr
 
-    def _stage_graph(self, plan: Plan, st, cfg_scale: float, masked: bool, ts_sampler: bool):
+    def _stage_graph(self, plan: Plan, st, cfg_scale: float, masked: bool, ts_sampler: bool, active=()):
         sid = plan.stage_ids.setdefault((st.lcs, st.ev), len(plan.stage_ids))   # exact structure -> id (no hash collisions)
-        name = f"stage:{sid}:{cfg_scale}:{int(masked)}{int(ts_sampler)}"
-        fn = lambda: plan.stage(st.lcs, st.ev, cfg_scale, masked, ts_sampler)  # noqa: E731
+        name = f"stage:{sid}:{cfg_scale}:{int(masked)}{int(ts_sampler)}" + self._control_name(plan, active)
+        fn = lambda: plan.stage(st.lcs, st.ev, cfg_scale, masked, ts_sampler, active)  # noqa: E731
         return name, fn, self._graph(plan, name, fn)
+
+    # ------------------------------------------------------------------------------------------ ControlNet
+    def _set_controls(self, plan: Plan, controls):
+        """controls: [(ControlNetWeights, hint uint8 [8h, 8w, 3], weight, guidance_start, guidance_end)], unit k in slot k.
+        Builds the slots' segments (dropping the graphs that ran a slot's previous model), runs each hint block and
+        scales the slots' zero convs; returns the (start, end) windows."""
+        if len(controls) > MAX_CONTROLS:
+            raise ValueError(f"{len(controls)} ControlNet units: at most {MAX_CONTROLS} are served")
+        windows = []
+        for slot, (cw, hint, weight, start, end) in enumerate(controls):
+            if not isinstance(cw, ControlNetWeights) or cw.cfg != self.unet_cfg:
+                raise ValueError(f"ControlNet {getattr(cw, 'name', cw)!r} does not match this engine's UNet")
+            if tuple(hint.shape) != (8 * plan.h, 8 * plan.w, 3) or hint.dtype != torch.uint8:
+                raise ValueError(f"control map {tuple(hint.shape)} {hint.dtype}: expected uint8 "
+                                 f"({8 * plan.h}, {8 * plan.w}, 3)")
+            if plan.unet.set_control(slot, cw, MAX_STEPS, plan.step):
+                for name in [n for n in plan.graphs if f"|cn{slot}=" in n]:
+                    del plan.graphs[name]
+                    plan.graph_launches.pop(name, None)
+            plan.unet.segments[slot].set_hint(hint.to(self.device), float(weight))
+            windows.append((float(start), float(end)))
+        return windows
+
+    def _active(self, i: int, n: int) -> tuple:
+        """slots whose unit is active at sampler step i of n: guidance_start <= i / n <= guidance_end"""
+        return tuple(s for s, (a, b) in enumerate(self._windows) if a <= i / n <= b)
+
+    @staticmethod
+    def _control_name(plan: Plan, active) -> str:
+        """graph-name suffix of the active slots and their models (empty without ControlNet: today's names)"""
+        return "".join(f"|cn{s}={plan.unet.segments[s].w.name}" for s in active)
+
+    def _control_tables(self, plan: Plan, ts: torch.Tensor):
+        """each unit's own time-embedding rows for the evaluations' timesteps"""
+        for s in range(len(self._windows)):
+            seg = plan.unet.segments[s]
+            seg.table[:ts.numel()].copy_(TimeEmbedding(seg.w).table(ts))
 
     @torch.no_grad()
     def run_program(self, cond: torch.Tensor, uncond: torch.Tensor, x_start: torch.Tensor, pr: "Program", cfg_scale: float,
-                    noises: Optional[torch.Tensor] = None, inpaint=None) -> torch.Tensor:
+                    noises: Optional[torch.Tensor] = None, inpaint=None, controls=None) -> torch.Tensor:
         """cond/uncond [b, 77 * k, ctx] on device (cond and uncond may have different k); x_start [b, 4, h, w] fp32 (host or device) = Program.start(...): the start
         latents in the sampler's own space; noises [pr.draws, b, 4, h, w]: the per-image N(0,1) draws after the first;
-        inpaint = (clean init latents [b, 4, h, w], latent mask [h * w]).  Returns the final latents fp32 [b, h*w, 4]
-        (NHWC, a view of plan state)."""
+        inpaint = (clean init latents [b, 4, h, w], latent mask [h * w]).  controls: ControlNet units, see _set_controls
+        (None: no ControlNet).  Returns the final latents fp32 [b, h*w, 4] (NHWC, a view of plan state)."""
         b, _, h, w = x_start.shape
         if pr.draws and (noises is None or noises.shape[0] < pr.draws):
             raise ValueError(f"{pr.sampler} needs {pr.draws} per-image noise draws")
@@ -602,6 +648,9 @@ class SDEngine:
         uncond = uncond if isinstance(uncond, Cond) else Cond(uncond)
         with self._ctx():
             plan = self.plan(b, h, w)
+            if controls and cond.y is not None:
+                raise ValueError("ControlNet is not served for SDXL")
+            self._windows = self._set_controls(plan, controls) if controls else []
             plan.set_context(cond.ctx, uncond.ctx)
             # SDXL: the vector conditioning of [cond | uncond] enters through the time-embedding table (per-sample rows)
             self._y = None if cond.y is None else torch.cat([cond.y, uncond.y]).to(self.device)
@@ -642,27 +691,36 @@ class SDEngine:
             return
         name = f"{pr.sampler if pr.fused != 'ddim' else 'DDIM'}:{cfg_scale}"
         if pr.fused == "ddim":
-            step_fn = (lambda: plan.step_ddim_masked(cfg_scale)) if masked else (lambda: plan.step_ddim(cfg_scale))
+            step_fn = (lambda a=(): plan.step_ddim_masked(cfg_scale, a)) if masked else \
+                (lambda a=(): plan.step_ddim(cfg_scale, a))
             name += ":mask" if masked else ""
         elif pr.fused == "euler_a":
             self._upload_noises(plan, noises[:n_evals])
             name = f"Euler a:{cfg_scale}"
-            step_fn = lambda: plan.step_euler_a(cfg_scale)  # noqa: E731
+            step_fn = lambda a=(): plan.step_euler_a(cfg_scale, a)  # noqa: E731
         elif pr.fused == "euler":
-            step_fn = lambda: plan.step_euler(cfg_scale)  # noqa: E731
+            step_fn = lambda a=(): plan.step_euler(cfg_scale, a)  # noqa: E731
         else:
-            step_fn = lambda: plan.step_dpmpp_2m(cfg_scale)  # noqa: E731
-        plan.table[:n_evals].copy_(self.temb.table(torch.tensor(pr.ts, dtype=torch.float32), self._y))
+            step_fn = lambda a=(): plan.step_dpmpp_2m(cfg_scale, a)  # noqa: E731
+        ts = torch.tensor(pr.ts, dtype=torch.float32)
+        plan.table[:n_evals].copy_(self.temb.table(ts, self._y))
+        self._control_tables(plan, ts)
         (plan.coef8 if len(pr.rows[0]) == 8 else plan.coef)[:n_evals].copy_(torch.tensor(pr.rows, dtype=torch.float32))
-        g = self._graph(plan, name, step_fn)
-        for _ in range(n_evals):
+        steps = {}   # active ControlNet slots -> (graph name, step function, graph); no units: () for every evaluation
+        for i in range(n_evals):
             if self.interrupted:
                 break
+            active = self._active(i, n_evals)
+            if active not in steps:
+                fn = (lambda a: lambda: step_fn(a))(active) if active else step_fn
+                gname = name + self._control_name(plan, active)
+                steps[active] = (gname, fn, self._graph(plan, gname, fn))
+            gname, fn, g = steps[active]
             if g is not None:
                 g.replay()
-                self.graph_replayed_launches += plan.graph_launches[name]
+                self.graph_replayed_launches += plan.graph_launches[gname]
             else:
-                step_fn()
+                fn()
             self.last_unet_evals += 1
 
     def _run_stages(self, plan: Plan, sp, cfg_scale: float, noises, masked: bool):
@@ -672,12 +730,16 @@ class SDEngine:
         if not stages:
             return
         self._upload_noises(plan, noises if noises is not None else torch.zeros((0, plan.b, 4, plan.h, plan.w)), sp.mix)
-        plan.table[:len(stages)].copy_(self.temb.table(torch.tensor([st.t for st in stages], dtype=torch.float32), self._y))
+        ts = torch.tensor([st.t for st in stages], dtype=torch.float32)
+        plan.table[:len(stages)].copy_(self.temb.table(ts, self._y))
+        self._control_tables(plan, ts)
         plan.coefL[:len(stages)].copy_(torch.tensor([st.row() for st in stages], dtype=torch.float32))
-        for st in stages:
+        step_of = S.stage_steps(stages)
+        for st, i in zip(stages, step_of):
             if self.interrupted:
                 break
-            name, fn, g = self._stage_graph(plan, st, cfg_scale, masked, sp.timestep_sampler)
+            name, fn, g = self._stage_graph(plan, st, cfg_scale, masked, sp.timestep_sampler,
+                                            self._active(i, step_of[-1] + 1))
             if g is not None:
                 g.replay()
                 self.graph_replayed_launches += plan.graph_launches[name]
@@ -695,6 +757,7 @@ class SDEngine:
         rtol, atol, order = 0.05, 0.0078, 3
         pid = S.PIDStepSizeController(0.05, 0.0, 1.0, 0.0, order, 0.81)
         s = t_start
+        accepted = 0   # the sampler step of an attempt (ControlNet windows: of the requested steps)
         x_prev = plan.x.clone()
         if plan.noise is None:
             plan.noise_rows(1)
@@ -703,12 +766,15 @@ class SDEngine:
                 break
             t = min(t_end, s + pid.h)
             stages = S.dpm_adaptive_attempt(s, t, t_of)
-            plan.table[:3].copy_(self.temb.table(torch.tensor([st.t for st in stages], dtype=torch.float32), self._y))
+            ts = torch.tensor([st.t for st in stages], dtype=torch.float32)
+            plan.table[:3].copy_(self.temb.table(ts, self._y))
+            self._control_tables(plan, ts)
             plan.coefL[:3].copy_(torch.tensor([st.row() for st in stages], dtype=torch.float32))
+            active = self._active(accepted, max(pr.steps, 1)) if self._windows else ()
             plan.step.zero_()
             ops.pack_unet_input(plan.x, plan.unet.xin, S.c_in(math.exp(-s)))
             for st in stages:
-                name, fn, g = self._stage_graph(plan, st, cfg_scale, masked, False)
+                name, fn, g = self._stage_graph(plan, st, cfg_scale, masked, False, active)
                 if g is not None:
                     g.replay()
                     self.graph_replayed_launches += plan.graph_launches[name]
@@ -722,6 +788,7 @@ class SDEngine:
                 x_prev.copy_(x_low)
                 plan.x.copy_(x_high)
                 s = t
+                accepted += 1
 
     @torch.no_grad()
     def sample(self, cond: torch.Tensor, uncond: torch.Tensor, x_T: torch.Tensor, steps: int, cfg_scale: float,
@@ -807,7 +874,7 @@ class SDEngine:
                 denoising_strength: float = 0.75, steps: int = 20, cfg_scale: float = 7.0, sampler: str = "DDIM",
                 scheduler: Optional[str] = None, latmask: Optional[torch.Tensor] = None,
                 inpainting_fill: int = 1, multipliers: Optional[torch.Tensor] = None,
-                neg_multipliers: Optional[torch.Tensor] = None) -> torch.Tensor:
+                neg_multipliers: Optional[torch.Tensor] = None, controls=None) -> torch.Tensor:
         """img2img: VAE-encode the init images (posterior mean), noise them to t_enc, run the remaining part of the
         sampler's schedule, decode.  init_u8 uint8 [b, H, W, 3].  Returns uint8 [b, H, W, 3] on device.
         `latmask` fp32 [h * w] (b200sd.inpaint.prepare_mask): inpainting — the region with latmask 0 is held to the init
@@ -816,7 +883,9 @@ class SDEngine:
         (inpaint.apply_overlays).
         `inpainting_fill` 2 ("latent noise") / 3 ("latent nothing") replace the repainted region of the init latents by
         the request's start noise / by zeros first (sdwui Img2Img.init); 0 ("fill") is image-space work the caller does
-        before the call (inpaint.fill_masked), 1 keeps the original content."""
+        before the call (inpaint.fill_masked), 1 keeps the original content.
+        `controls`: ControlNet units [(ControlNetWeights, control map uint8 [H, W, 3], weight, guidance_start,
+        guidance_end)], at most 3 (None: none)."""
         b = tokens.shape[0]
         cond, uncond = self._conds(tokens, neg_tokens, init_u8.shape[2], init_u8.shape[1], multipliers, neg_multipliers)
         init = self.encode(init_u8)
@@ -827,11 +896,11 @@ class SDEngine:
             if inpainting_fill == 2:   # create_random_tensors(shape, seeds): the same first draw the sampler starts from
                 init = init + per_image_noise(seed, b, (4, h, w), 1, *self.variation)[0].to(self.device) * nm
         lat = self._sample_from(init, cond, uncond, seed, denoising_strength, steps, cfg_scale, sampler, scheduler,
-                                inpaint=None if latmask is None else (init, latmask))
+                                inpaint=None if latmask is None else (init, latmask), controls=controls)
         return self.decode(lat, h, w)
 
     def _sample_from(self, init: torch.Tensor, cond, uncond, seed: int, denoising_strength: float, steps: int,
-                     cfg_scale: float, sampler: str, scheduler: Optional[str], inpaint=None) -> torch.Tensor:
+                     cfg_scale: float, sampler: str, scheduler: Optional[str], inpaint=None, controls=None) -> torch.Tensor:
         """the img2img half of a sampler (also the second pass of the hires fix): `init` [b, 4, h, w] latents on the device,
         fresh per-image noise from `seed`, start at the noise level of t_enc.
         DDIM / PLMS: sdwui sd_samplers_timesteps.sample_img2img; k-diffusion samplers: KDiffusionSampler.sample_img2img."""
@@ -839,7 +908,7 @@ class SDEngine:
         pr = self.program(sampler, scheduler, steps, denoise=denoising_strength, masked=inpaint is not None)
         nz = per_image_noise(seed, b, (4, h, w), 1 + pr.draws, *self.variation)
         return self.run_program(cond, uncond, pr.start(nz[0].to(self.device), init), pr, cfg_scale,
-                                noises=nz[1:] if pr.draws else None, inpaint=inpaint)
+                                noises=nz[1:] if pr.draws else None, inpaint=inpaint, controls=controls)
 
     @torch.no_grad()
     def txt2img_hires(self, tokens: torch.Tensor, neg_tokens: torch.Tensor, seed: int, steps: int = 20,
@@ -866,19 +935,22 @@ class SDEngine:
         return self.decode(lat2, h2, w2)
 
     def _sample_txt(self, cond, uncond, seed: int, b: int, h: int, w: int, steps: int, cfg_scale: float, sampler: str,
-                    scheduler: Optional[str]) -> torch.Tensor:
+                    scheduler: Optional[str], controls=None) -> torch.Tensor:
         pr = self.program(sampler, scheduler, steps)
         nz = per_image_noise(seed, b, (4, h, w), 1 + pr.draws, *self.variation)
-        return self.run_program(cond, uncond, pr.start(nz[0]), pr, cfg_scale, noises=nz[1:] if pr.draws else None)
+        return self.run_program(cond, uncond, pr.start(nz[0]), pr, cfg_scale, noises=nz[1:] if pr.draws else None,
+                                controls=controls)
 
     @torch.no_grad()
     def txt2img(self, tokens: torch.Tensor, neg_tokens: torch.Tensor, seed: int, steps: int = 20, cfg_scale: float = 7.0,
                 height: int = 512, width: int = 512, sampler: str = "DDIM", scheduler: Optional[str] = None,
-                multipliers: Optional[torch.Tensor] = None, neg_multipliers: Optional[torch.Tensor] = None) -> torch.Tensor:
+                multipliers: Optional[torch.Tensor] = None, neg_multipliers: Optional[torch.Tensor] = None,
+                controls=None) -> torch.Tensor:
         """Whole request for this engine's share: returns uint8 [b, H, W, 3] on device.  tokens [b, 77 * k] and
-        neg_tokens [b, 77 * k'] with their optional emphasis multipliers of the same shapes (factory.tokenize_prompts)."""
+        neg_tokens [b, 77 * k'] with their optional emphasis multipliers of the same shapes (factory.tokenize_prompts).
+        `controls`: ControlNet units as for img2img (None: none)."""
         b = tokens.shape[0]
         h, w = height // 8, width // 8
         cond, uncond = self._conds(tokens, neg_tokens, width, height, multipliers, neg_multipliers)
-        lat = self._sample_txt(cond, uncond, seed, b, h, w, steps, cfg_scale, sampler, scheduler)
+        lat = self._sample_txt(cond, uncond, seed, b, h, w, steps, cfg_scale, sampler, scheduler, controls)
         return self.decode(lat, h, w)

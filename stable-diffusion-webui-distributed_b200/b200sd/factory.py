@@ -4,18 +4,21 @@ Weights: `SD_CKPT=/path/model.safetensors` (ldm key names; read for sd15 and sd2
 synthetic weights of synth.py (no checkpoint exists offline — every benchmark / parity number in this repo uses those).
 Model family: B200SD_MODEL = sd15 (default) | sdxl | sd21 | tiny | tinyxl | tiny21.  Prediction type: each family's
 default (v for sd21 / tiny21, eps for the others), overridden by B200SD_PREDICTION = eps | v.
+ControlNets (controlnet()): B200SD_CONTROLNET_DIR/<model>.safetensors, otherwise seeded synthetic weights.
 """
 import logging
 import os
 import threading
 import zlib
+from collections import OrderedDict
 from typing import Dict, List, Optional, Tuple
 
 import torch
 
 from . import config as C
 from .engine import SDEngine
-from .synth import make_state_dict
+from .synth import make_controlnet_state_dict, make_state_dict
+from .unet_exec import ControlNetWeights
 
 log = logging.getLogger("distributed")
 _LOCK = threading.Lock()
@@ -91,13 +94,54 @@ def default_engine_factory(device: str, size: str = None) -> SDEngine:
 
 
 def evict(device: str) -> int:
-    """forget the cached engines of `device` (LocalGPUWorker.restart): their weights, plans and graphs are freed once the
-    last reference goes"""
+    """forget the cached engines and ControlNets of `device` (LocalGPUWorker.restart): their weights, plans and graphs
+    are freed once the last reference goes"""
     with _LOCK:
         keys = [k for k in _ENGINES if k.startswith(f"{device}:")]
         for k in keys:
             _ENGINES.pop(k).release()
+        for k in [k for k in _CONTROLNETS if k[0] == str(device)]:
+            del _CONTROLNETS[k]
     return len(keys)
+
+
+MAX_CONTROLNETS = 3   # packed ControlNet models kept per device; the least recently used one is dropped beyond that
+_CONTROLNETS: "OrderedDict[tuple, ControlNetWeights]" = OrderedDict()
+
+
+def _controlnet_state(name: str, size: str) -> Dict[str, torch.Tensor]:
+    """B200SD_CONTROLNET_DIR/<name>.safetensors (ldm ControlNet keys, with or without `control_model.`), or seeded
+    synthetic weights (crc32 of the name) when the variable is not set"""
+    root = os.environ.get("B200SD_CONTROLNET_DIR")
+    if not root:
+        log.warning("b200sd: B200SD_CONTROLNET_DIR is not set — ControlNet %r uses SEEDED SYNTHETIC weights; set it to a "
+                    "directory of <model>.safetensors files for real ControlNets", name)
+        return make_controlnet_state_dict(configs(size)[0], seed=zlib.crc32(name.encode("utf-8")))
+    path = os.path.join(root, name + ".safetensors")
+    if not os.path.isfile(path):
+        raise FileNotFoundError(f"ControlNet model {name!r} not found: no {path}")
+    sd = _load_safetensors(path)
+    if any(k.startswith(("controlnet_cond_embedding.", "controlnet_down_blocks.")) for k in sd):
+        raise ValueError(f"{path} is a diffusers-layout ControlNet: only ldm ControlNet checkpoints are served")
+    return {(k if k.startswith(C.CONTROL_PREFIX) else C.CONTROL_PREFIX + k): v for k, v in sd.items()}
+
+
+def controlnet(name: str, size: str = None, device: str = "cuda:0", dtype=torch.float16) -> ControlNetWeights:
+    """ControlNet `name` for the `size` family (default B200SD_MODEL), packed on `device` and cached there"""
+    size = size or os.environ.get("B200SD_MODEL", "sd15")
+    key = (str(device), size, name, os.environ.get("B200SD_CONTROLNET_DIR", ""), dtype)
+    with _LOCK:
+        cw = _CONTROLNETS.get(key)
+        if cw is not None:
+            _CONTROLNETS.move_to_end(key)
+            return cw
+    cw = ControlNetWeights(_controlnet_state(name, size), configs(size)[0], torch.device(device), dtype, name=name)
+    with _LOCK:
+        _CONTROLNETS[key] = cw
+        mine = [k for k in _CONTROLNETS if k[0] == str(device)]
+        for k in mine[:max(0, len(mine) - MAX_CONTROLNETS)]:
+            del _CONTROLNETS[k]
+    return cw
 
 
 def model_identity(size: str = None) -> str:

@@ -341,6 +341,17 @@ def image_to_nhwc(img_u8: torch.Tensor, out: torch.Tensor):
     return out
 
 
+def hint_to_nhwc(img_u8: torch.Tensor, out: torch.Tensor):
+    """img_u8 uint8 [B, HW, 3] -> out [B, HW, pitch]: channels 0..2 = x/255, the rest of the row 0 (ControlNet hint)"""
+    b, hw, _ = img_u8.shape
+    assert img_u8.dtype == torch.uint8 and img_u8.is_contiguous()
+    assert out.shape[:2] == (b, hw) and out.stride(2) == 1 and out.stride(0) == hw * out.stride(1)
+    rc = _lib.lib().b200sd_hint_to_nhwc(_p(img_u8), _p(out), ctypes.c_longlong(out.stride(1)), b, hw, _dt(out), _stream())
+    check(rc, "b200sd_hint_to_nhwc")
+    _count()
+    return out
+
+
 def unpack_latent(moments: torch.Tensor, x: torch.Tensor, scale: float):
     """moments [B, HW, pitch] (first 4 channels = posterior mean) -> x fp32 [B, HW, 4] = mean * scale"""
     b, hw, _ = moments.shape

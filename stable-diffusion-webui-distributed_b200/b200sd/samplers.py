@@ -68,6 +68,17 @@ class SamplerPlan:
     timestep_sampler: bool = False   # DDIM / PLMS: inpainting masks blend the evaluated tensor BEFORE the model call
 
 
+def stage_steps(stages: Sequence[Stage]) -> List[int]:
+    """the sampler step of every stage (ControlNet guidance windows): a step begins with each evaluation of the step's
+    own latent x (ev "x"); evaluations of intermediate points (ev "u": Heun's x_2, DPM2's midpoint, the inner stages of
+    DPM-Solver and PLMS's warm-up) belong to the step in progress"""
+    out, i = [], -1
+    for st in stages:
+        i += st.ev == "x"
+        out.append(max(i, 0))
+    return out
+
+
 def c_in(sigma: float) -> float:
     return 1.0 / math.sqrt(sigma * sigma + 1.0)
 

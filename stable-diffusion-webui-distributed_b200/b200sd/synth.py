@@ -9,8 +9,8 @@ from typing import Dict
 
 import torch
 
-from .config import (CLIP_PREFIX, OPENCLIP_PREFIX, UNET_PREFIX, VAE_PREFIX, XL_PREFIX0, XL_PREFIX1, CLIPConfig,
-                     UNetConfig, VAEConfig, unet_layout)
+from .config import (CLIP_PREFIX, CONTROL_PREFIX, OPENCLIP_PREFIX, UNET_PREFIX, VAE_PREFIX, XL_PREFIX0, XL_PREFIX1,
+                     CLIPConfig, UNetConfig, VAEConfig, controlnet_layout, unet_layout)
 
 
 class _Init:
@@ -41,8 +41,7 @@ class _Init:
             self.b(key + ".bias", cout)
 
 
-def _unet(i: _Init, cfg: UNetConfig):
-    p = UNET_PREFIX
+def _unet(i: _Init, cfg: UNetConfig, p: str = UNET_PREFIX, encoder_only: bool = False):
     ted = cfg.time_embed_dim
     i.lin(p + "time_embed.0", ted, cfg.model_channels)
     i.lin(p + "time_embed.2", ted, ted)
@@ -99,10 +98,30 @@ def _unet(i: _Init, cfg: UNetConfig):
     for n, layers in enumerate(inputs):
         block(f"input_blocks.{n}", layers)
     block("middle_block", middle)
+    if encoder_only:
+        return
     for n, layers in enumerate(outputs):
         block(f"output_blocks.{n}", layers)
     i.norm(p + "out.0", cfg.model_channels)
     i.conv(p + "out.2", cfg.out_channels, cfg.model_channels, 3)
+
+
+def make_controlnet_state_dict(unet: UNetConfig, seed: int = 0) -> Dict[str, torch.Tensor]:
+    """An ldm ControlNet for a UNet of config `unet`, with the key names of ControlNet checkpoints (control_model.*):
+    time_embed, the UNet's input_blocks and middle_block, input_hint_block.{0,2,..,14}, zero_convs.i.0 and
+    middle_block_out.0.  Zero convs are initialised like any other layer (ldm zero-inits them), so a synthetic unit
+    changes the image."""
+    i = _Init(seed)
+    p = CONTROL_PREFIX
+    _unet(i, unet, p, encoder_only=True)
+    _, _, hint, zero_ch = controlnet_layout(unet)
+    for j, (cin, cout, _) in enumerate(hint):
+        i.conv(f"{p}input_hint_block.{2 * j}", cout, cin, 3)
+    for j, c in enumerate(zero_ch):
+        i.conv(f"{p}zero_convs.{j}.0", c, c, 1)
+    mid = zero_ch[-1]
+    i.conv(p + "middle_block_out.0", mid, mid, 1)
+    return i.sd
 
 
 def _vae(i: _Init, cfg: VAEConfig):

@@ -16,13 +16,17 @@ from the reference at scripts/spartan/world.py:196 and, remotely, worker.py:432)
   * q/k/v projection weights carry zero rows so each head is padded to a multiple of 64 columns — exactly one
     TMA SWIZZLE_128B box per head chunk in the attention kernel.
 """
-from typing import Dict, List
+import contextlib
+from typing import Dict, List, Optional
 
 import torch
 
 from . import ops
-from .config import UNET_PREFIX, UNetConfig, unet_layout
+from .config import CONTROL_PREFIX, UNET_PREFIX, UNetConfig, controlnet_layout, unet_layout
 from .weights import pack_conv, pack_geglu, pad_heads
+
+
+MAX_CONTROLS = 3   # ControlNet units per request (sd-webui-controlnet's default unit count)
 
 
 def _pad64(d: int) -> int:
@@ -59,10 +63,12 @@ class Pool:
 
 class UNetWeights:
     """Packs an ldm state_dict (fp32, any device) into kernel layouts on `device`."""
+    PREFIX = UNET_PREFIX
+    ENCODER_ONLY = False   # time embedding, input blocks and middle block only (ControlNetWeights)
 
     def __init__(self, sd: Dict[str, torch.Tensor], cfg: UNetConfig, device, dtype=torch.float16):
         self.cfg, self.device, self.dtype = cfg, device, dtype
-        self.p = UNET_PREFIX
+        self.p = self.PREFIX
         self.sd = sd
         self.t: Dict[str, torch.Tensor] = {}
         self.layout = unet_layout(cfg)
@@ -174,15 +180,50 @@ class UNetWeights:
         for n, layers in enumerate(inputs):
             block(f"input_blocks.{n}", layers)
         block("middle_block", middle)
-        for n, layers in enumerate(outputs):
-            block(f"output_blocks.{n}", layers)
-        self._norm("out.gn", "out.0")
-        self._conv("out.conv", "out.2", cout_pad=32)
+        if not self.ENCODER_ONLY:
+            for n, layers in enumerate(outputs):
+                block(f"output_blocks.{n}", layers)
+            self._norm("out.gn", "out.0")
+            self._conv("out.conv", "out.2", cout_pad=32)
+        self._pack_extra()
         self.t["emb_all.w"] = self._dev(torch.cat(emb_w))
         self.t["emb_all.b"] = self._dev(torch.cat(emb_b), torch.float32)
         self.t["conv1_bias_all"] = self._dev(torch.cat(conv1_b), torch.float32)
         self.emb_total = off
         self.sd = None  # drop the reference to the fp32 dict
+
+    def _pack_extra(self):
+        """layers a subclass adds to the UNet's (ControlNetWeights: hint block and zero convs)"""
+
+
+def _pad_to(c: int, m: int) -> int:
+    return -(-c // m) * m
+
+
+class ControlNetWeights(UNetWeights):
+    """An ldm ControlNet (keys `control_model.*`, factory.controlnet) packed for a UNet of config `cfg`: its time
+    embedding, input blocks and middle block go through UNetWeights' packers under the same names (`input_blocks.1.0.
+    conv1.w`, `emb_all.w`, ...), plus
+      hint.j.w / .b   input_hint_block conv j (3x3; input channels padded to a multiple of 64, outputs to one of 32, as
+                      conv_in and out.conv are padded: the padded weights are zero)
+      zero.i.w / .b   zero conv i (1x1, a linear over channels); zero.mid the middle_block_out conv.
+    `name` identifies the model in graph names and caches."""
+    PREFIX = CONTROL_PREFIX
+    ENCODER_ONLY = True
+
+    def __init__(self, sd: Dict[str, torch.Tensor], cfg: UNetConfig, device, dtype=torch.float16, name: str = "control"):
+        self.name = name
+        self.hint_layout = controlnet_layout(cfg)[2]
+        super().__init__(sd, cfg, device, dtype)
+
+    def _pack_extra(self):
+        _, _, hint, zero_ch = controlnet_layout(self.cfg)
+        for j, (cin, cout, _) in enumerate(hint):
+            self._conv(f"hint.{j}", f"input_hint_block.{2 * j}", cin_pad=_pad_to(cin, 64), cout_pad=_pad_to(cout, 32))
+        for i in range(len(zero_ch)):
+            self._lin(f"zero.{i}", f"zero_convs.{i}.0")
+        self._lin("zero.mid", "middle_block_out.0")
+        self.n_zero = len(zero_ch)
 
 
 class UNetProgram:
@@ -212,6 +253,7 @@ class UNetProgram:
         self.ops: List = []
         self.op_flops: List = []
         self.gn_elems = self.ln_elems = 0     # elements normalised per evaluation (bench.py's HBM roofline)
+        self.segments: List[Optional["ControlSegment"]] = [None] * MAX_CONTROLS   # ControlNet unit slots
         self._build()
         # one statistics buffer serves every GroupNorm (they run back to back on one stream); zeroed once, here
         self.stats_all = torch.zeros((max(1, self.gn_need),), device=self.dev, dtype=torch.float32)
@@ -232,8 +274,9 @@ class UNetProgram:
             ctx = torch.cat([ctx, ctx.new_zeros((n, self.ctx_len - l, c))], dim=1)
         l = self.ctx_len
         ctx2 = ctx.reshape(n * l, c)
-        for key, buf in self.ctx_kv.items():
-            ops.linear(ctx2, self.w.t[key + ".attn2.kv.w"], buf.reshape(n * l, -1), bias=self.w.t[key + ".attn2.kv.b"])
+        for w, ctx_kv in [(self.w, self.ctx_kv)] + [(s.w, s.ctx_kv) for s in self.segments if s is not None]:
+            for key, buf in ctx_kv.items():
+                ops.linear(ctx2, w.t[key + ".attn2.kv.w"], buf.reshape(n * l, -1), bias=w.t[key + ".attn2.kv.b"])
         if self.ctx_len != self.ctx_len0:
             self.kv_len.copy_(torch.tensor(lengths, dtype=torch.int32))
 
@@ -243,13 +286,85 @@ class UNetProgram:
         hold the old buffers' addresses: the caller drops them."""
         assert cap > self.ctx_len
         self.ctx_len = cap
-        for tb in list(self.ctx_kv):
-            old = self.ctx_kv[tb]
-            self.ctx_kv[tb] = torch.zeros((self.n, cap, old.shape[2]), device=self.dev, dtype=self.dt)
-        for i, tb, q2, o, heads, d, dp, scale in self._xattn:
-            kv = self.ctx_kv[tb]
-            self.ops[i] = (ops.attention, (q2, kv[..., :heads * dp], kv[..., heads * dp:], o, heads, d, dp, scale, dp > d),
-                           {"kv_len": self.kv_len})
+        for ctx_kv, xattn, op_list in [(self.ctx_kv, self._xattn, self.ops)] + \
+                [(s.ctx_kv, s.xattn, s.ops) for s in self.segments if s is not None]:
+            for tb in list(ctx_kv):
+                old = ctx_kv[tb]
+                ctx_kv[tb] = torch.zeros((self.n, cap, old.shape[2]), device=self.dev, dtype=self.dt)
+            self._varlen_xattn(ctx_kv, xattn, op_list)
+
+    def _varlen_xattn(self, ctx_kv, xattn, op_list):
+        """point the attn2 launches listed in `xattn` at the K/V buffers of `ctx_kv`, with per-row key counts"""
+        for i, tb, q2, o, heads, d, dp, scale in xattn:
+            kv = ctx_kv[tb]
+            op_list[i] = (ops.attention, (q2, kv[..., :heads * dp], kv[..., heads * dp:], o, heads, d, dp, scale, dp > d),
+                          {"kv_len": self.kv_len})
+
+    # ---------------------------------------------------------------- ControlNet
+    def set_control(self, slot: int, cw: "ControlNetWeights", table_rows: int, step: torch.Tensor) -> bool:
+        """Make unit slot `slot` (0 .. MAX_CONTROLS-1) run ControlNet `cw`, its time-embedding rows selected by the
+        device counter `step`: builds the slot's segment unless it already holds that model.  Returns True when it built
+        one (graphs that ran the slot's old segment are then stale)."""
+        if self.per_sample:
+            raise ValueError("ControlNet is not served for SDXL")
+        seg = self.segments[slot]
+        if seg is not None and seg.w is cw:
+            return False
+        self.segments[slot] = None   # the old segment's buffers go before the new ones are allocated
+        self.segments[slot] = ControlSegment(self, cw, table_rows, step)
+        return True
+
+    @contextlib.contextmanager
+    def emitting_into(self, seg: "ControlSegment"):
+        """the emitters (_run_layers, _res, _attn) build `seg`'s ops: its weights, biases, K/V buffers and op list stand in
+        for the UNet's, and the element counters of the UNet's roofline stay as they are"""
+        saved = (self.w, self.cur_bias, self.ctx_kv, self._xattn, self.ops, self.op_flops, self.gn_elems, self.ln_elems)
+        self.w, self.cur_bias, self.ctx_kv, self._xattn, self.ops, self.op_flops = \
+            seg.w, seg.cur_bias, seg.ctx_kv, seg.xattn, seg.ops, seg.op_flops
+        try:
+            yield
+        finally:
+            (self.w, self.cur_bias, self.ctx_kv, self._xattn, self.ops, self.op_flops, self.gn_elems,
+             self.ln_elems) = saved
+
+    def _run_layers(self, prefix, layers, x, h, wd, final_dest, conv_in_residual=None):
+        """x: input view; the LAST layer writes into final_dest (a view with the right channel count).  conv_in reads the
+        program's input xin; `conv_in_residual` (a ControlNet's hint features) is added in its epilogue."""
+        cfg, n, t = self.cfg, self.n, self.w.t
+        prev_tmp = None
+        for li, layer in enumerate(layers):
+            key = f"{prefix}.{li}"
+            last = li == len(layers) - 1
+            kind = layer[0]
+            tmp = None
+            if kind == "conv_in":
+                dest = final_dest
+                self._emit(ops.conv2d, self.xin.unflatten(1, (h, wd)), t[key + ".w"], dest, ksize=3, bias=t[key + ".b"],
+                           residual=conv_in_residual, algo_flops=2.0 * n * h * wd * 9 * cfg.in_channels * layer[2])
+            elif kind == "res":
+                dest = final_dest if last else self.pool.get(n, h * wd, layer[2])
+                tmp = None if last else dest
+                self._res(key, x, layer[1], layer[2], h, wd, dest)
+            elif kind == "attn":
+                dest = final_dest if last else self.pool.get(n, h * wd, layer[1])
+                tmp = None if last else dest
+                self._attn(key, x, layer[1], layer[2], h, wd, dest)
+            elif kind == "down":
+                dest = final_dest
+                self._emit(ops.conv2d, x.unflatten(1, (h, wd)), t[key + ".w"], dest, ksize=3, stride=2, bias=t[key + ".b"])
+                h, wd = (h + 1) // 2, (wd + 1) // 2
+            elif kind == "up":
+                up = self.pool.get(n, 4 * h * wd, layer[1])
+                self._emit(ops.upsample2x, x.unflatten(1, (h, wd)), up.unflatten(1, (2 * h, 2 * wd)))
+                h, wd = 2 * h, 2 * wd
+                dest = final_dest
+                self._emit(ops.conv2d, up.unflatten(1, (h, wd)), t[key + ".w"], dest, ksize=3, bias=t[key + ".b"])
+                self.pool.put(up)
+            if prev_tmp is not None:  # the previous layer's scratch output has now been consumed
+                self.pool.put(prev_tmp)
+            prev_tmp = tmp
+            x = dest
+        return x, h, wd
 
     # ---------------------------------------------------------------- program construction
     def _emit(self, fn, *a, algo_flops=None, **k):
@@ -373,51 +488,19 @@ class UNetProgram:
             c = cats[i]
             return c[..., c.shape[-1] - in_out_ch[j]:]
 
-        def run_layers(prefix, layers, x, h, wd, final_dest):
-            """x: input view; the LAST layer writes into final_dest (a view with the right channel count)."""
-            prev_tmp = None
-            for li, layer in enumerate(layers):
-                key = f"{prefix}.{li}"
-                last = li == len(layers) - 1
-                kind = layer[0]
-                tmp = None
-                if kind == "conv_in":
-                    dest = final_dest
-                    self._emit(ops.conv2d, self.xin.unflatten(1, (h, wd)), t[key + ".w"], dest, ksize=3, bias=t[key + ".b"],
-                               algo_flops=2.0 * n * h * wd * 9 * cfg.in_channels * layer[2])
-                elif kind == "res":
-                    dest = final_dest if last else self.pool.get(n, h * wd, layer[2])
-                    tmp = None if last else dest
-                    self._res(key, x, layer[1], layer[2], h, wd, dest)
-                elif kind == "attn":
-                    dest = final_dest if last else self.pool.get(n, h * wd, layer[1])
-                    tmp = None if last else dest
-                    self._attn(key, x, layer[1], layer[2], h, wd, dest)
-                elif kind == "down":
-                    dest = final_dest
-                    self._emit(ops.conv2d, x.unflatten(1, (h, wd)), t[key + ".w"], dest, ksize=3, stride=2, bias=t[key + ".b"])
-                    h, wd = (h + 1) // 2, (wd + 1) // 2
-                elif kind == "up":
-                    up = self.pool.get(n, 4 * h * wd, layer[1])
-                    self._emit(ops.upsample2x, x.unflatten(1, (h, wd)), up.unflatten(1, (2 * h, 2 * wd)))
-                    h, wd = 2 * h, 2 * wd
-                    dest = final_dest
-                    self._emit(ops.conv2d, up.unflatten(1, (h, wd)), t[key + ".w"], dest, ksize=3, bias=t[key + ".b"])
-                    self.pool.put(up)
-                if prev_tmp is not None:  # the previous layer's scratch output has now been consumed
-                    self.pool.put(prev_tmp)
-                prev_tmp = tmp
-                x = dest
-            return x, h, wd
-
         # ---- input blocks
         h, wd = self.h, self.wd
         x = None
         for j, layers in enumerate(inputs):
-            x, h, wd = run_layers(f"input_blocks.{j}", layers, x, h, wd, skip_slot(j))
+            x, h, wd = self._run_layers(f"input_blocks.{j}", layers, x, h, wd, skip_slot(j))
         # ---- middle block -> first concat buffer's h slot
         c0 = cats[0]
-        x, h, wd = run_layers("middle_block", middle, x, h, wd, c0[..., :c0.shape[-1] - in_out_ch[n_in - 1]])
+        x, h, wd = self._run_layers("middle_block", middle, x, h, wd, c0[..., :c0.shape[-1] - in_out_ch[n_in - 1]])
+        # ControlNet segments run here, between the middle block and the decoder: every pool buffer is free at this point,
+        # so a segment shares the pool; their outputs are added in place into these views, the skips and the middle result
+        self.mid_op = len(self.ops)
+        self.control_dest = [skip_slot(j) for j in range(n_in)] + [c0[..., :c0.shape[-1] - in_out_ch[n_in - 1]]]
+        self.in_res = in_res
         # ---- output blocks
         final = torch.empty((n, self.h * self.wd, cfg.model_channels), device=self.dev, dtype=self.dt)
         for i, layers in enumerate(outputs):
@@ -428,7 +511,7 @@ class UNetProgram:
                 dest = nxt[..., :nxt.shape[-1] - in_out_ch[n_in - 2 - i]]
             else:
                 dest = final
-            x, h, wd = run_layers(f"output_blocks.{i}", layers, cat, hh, ww, dest)
+            x, h, wd = self._run_layers(f"output_blocks.{i}", layers, cat, hh, ww, dest)
         # ---- out: GN + SiLU + conv3x3 -> eps (4 channels padded to 32)
         a = self.pool.get(n, self.h * self.wd, cfg.model_channels)
         self._gn(final, a, "out.gn", 1e-5, True)
@@ -437,9 +520,110 @@ class UNetProgram:
         self.pool.put(a)
 
     # ---------------------------------------------------------------- execution
-    def run(self):
-        for fn, a, k in self.ops:
+    def run(self, active=()):
+        """one evaluation; `active`: the ControlNet slots whose segments run (between the middle block and the decoder)"""
+        if not active:
+            for fn, a, k in self.ops:
+                fn(*a, **k)
+            return
+        for fn, a, k in self.ops[:self.mid_op]:
             fn(*a, **k)
+        for slot in active:
+            for fn, a, k in self.segments[slot].ops:
+                fn(*a, **k)
+        for fn, a, k in self.ops[self.mid_op:]:
+            fn(*a, **k)
+
+
+class ControlSegment:
+    """ControlNet unit slot of a UNetProgram (ldm ControlNet as sd-webui-controlnet drives it, Balanced mode).
+
+    `ops` is one evaluation of the ControlNet on the UNet's own input xin, timestep and contexts, run between the UNet's
+    middle block and its decoder (UNetProgram.run(active)): select this step's conv1 biases from `table`; conv_in with the
+    hint features as its epilogue residual; the input blocks and the middle block through the UNet's own emitters and
+    pool; after each block its zero conv, as a linear whose output and residual are the UNet's skip slice (or middle
+    result) — an in-place add into the concat buffer (b200sd_epilogue: residual == D).  The zero-conv weights are this
+    slot's copies, scaled by the unit's weight in set_hint, so a new weight needs no new graph.
+
+    `hint_ops` is the hint block on one image at the generation size (8h x 8w), run once per request by set_hint; its
+    [1, h*w, model_channels] output is broadcast to the [n, h*w, model_channels] features every batch row reads."""
+
+    def __init__(self, prog: UNetProgram, cw: "ControlNetWeights", table_rows: int, step: torch.Tensor):
+        self.w = cw
+        n, dev, dt = prog.n, prog.dev, prog.dt
+        self.n = n
+        self.cur_bias = torch.zeros((cw.emb_total,), device=dev, dtype=torch.float32)
+        self.table = torch.zeros((table_rows, cw.emb_total), device=dev, dtype=torch.float32)   # TimeEmbedding(cw) rows
+        self.hint_feat = torch.zeros((n, prog.h * prog.wd, cw.cfg.model_channels), device=dev, dtype=dt)
+        names = [f"zero.{i}" for i in range(cw.n_zero)] + ["zero.mid"]
+        self.zero = [(torch.zeros_like(cw.t[k + ".w"]), torch.zeros_like(cw.t[k + ".b"]), k) for k in names]
+        self.ctx_kv: Dict[str, torch.Tensor] = {}
+        self.xattn: List[tuple] = []
+        self.ops: List = []
+        self.op_flops: List = []
+        self._build(prog, step)
+        self._build_hint(prog)
+
+    def _build(self, prog: UNetProgram, step: torch.Tensor):
+        inputs, middle, _ = self.w.layout
+        n, zc = self.n, self.zero
+        holders = len(prog.gn_stats)
+        with prog.emitting_into(self):
+            prog._emit(ops.select_step, self.table, step, self.cur_bias)
+            h, wd = prog.h, prog.wd
+            x = prev = None
+            for j, layers in enumerate(inputs):
+                hh, ww = prog.in_res[j]
+                dest = prog.pool.get(n, hh * ww, prog.control_dest[j].shape[-1])
+                x, h, wd = prog._run_layers(f"input_blocks.{j}", layers, x, h, wd, dest,
+                                            conv_in_residual=self.hint_feat if j == 0 else None)
+                skip = prog.control_dest[j]
+                prog._emit(ops.linear, dest, zc[j][0], skip, bias=zc[j][1], residual=skip)
+                if prev is not None:
+                    prog.pool.put(prev)
+                prev = dest
+            mid = prog.pool.get(n, h * wd, prog.control_dest[-1].shape[-1])
+            x, h, wd = prog._run_layers("middle_block", middle, x, h, wd, mid)
+            prog.pool.put(prev)
+            out = prog.control_dest[-1]
+            prog._emit(ops.linear, mid, zc[-1][0], out, bias=zc[-1][1], residual=out)
+            prog.pool.put(mid)
+        assert prog.gn_need <= prog.stats_all.numel(), "a ControlNet GroupNorm needs more statistics than the UNet's"
+        for holder in prog.gn_stats[holders:]:
+            holder[0] = prog.stats_all
+        if prog.ctx_len != prog.ctx_len0:
+            prog._varlen_xattn(self.ctx_kv, self.xattn, self.ops)
+
+    def _build_hint(self, prog: UNetProgram):
+        cw, dev, dt = self.w, prog.dev, prog.dt
+        hh, ww = 8 * prog.h, 8 * prog.wd
+        cin_pads = [_pad_to(cin, 64) for cin, _, _ in cw.hint_layout]
+        self.hint_u8 = torch.zeros((1, hh * ww, 3), device=dev, dtype=torch.uint8)
+        cur = torch.zeros((1, hh * ww, cin_pads[0]), device=dev, dtype=dt)
+        self.hint_ops = [(ops.hint_to_nhwc, (self.hint_u8, cur), {})]
+        last = len(cw.hint_layout) - 1
+        for j, (_, cout, stride) in enumerate(cw.hint_layout):
+            cp = _pad_to(cout, 32)
+            ho, wo = (hh + 1) // 2 if stride == 2 else hh, (ww + 1) // 2 if stride == 2 else ww
+            # zero from allocation beyond the cp written channels: the next conv's padded input channels
+            out = torch.zeros((1, ho * wo, cp if j == last else max(cp, cin_pads[j + 1])), device=dev, dtype=dt)
+            self.hint_ops.append((ops.conv2d, (cur[..., :cin_pads[j]].unflatten(1, (hh, ww)), cw.t[f"hint.{j}.w"],
+                                               out[..., :cp]),
+                                  dict(ksize=3, stride=stride, bias=cw.t[f"hint.{j}.b"],
+                                       flags=0 if j == last else ops.EPI_SILU)))
+            cur, hh, ww = out, ho, wo
+        assert (hh, ww) == (prog.h, prog.wd) and cur.shape[-1] == cw.cfg.model_channels
+        self.hint_out = cur
+
+    def set_hint(self, hint_u8: torch.Tensor, weight: float):
+        """per request: the control map uint8 [8h, 8w, 3] (RGB, at the generation size) and the unit's weight"""
+        self.hint_u8.copy_(hint_u8.reshape(1, -1, 3))
+        for fn, a, k in self.hint_ops:
+            fn(*a, **k)
+        self.hint_feat.copy_(self.hint_out.expand(self.n, -1, -1))
+        for wt, b, key in self.zero:
+            wt.copy_(self.w.t[key + ".w"].float() * weight)
+            b.copy_(self.w.t[key + ".b"] * weight)
 
 
 class TimeEmbedding:

@@ -66,7 +66,7 @@ class LocalGPUWorker(Worker):
         return ok
 
     def query_scripts(self) -> dict:
-        return {"txt2img": [], "img2img": []}
+        return {"txt2img": ["controlnet"], "img2img": ["controlnet"]}
 
     def load_options(self, model, vae=None):
         """weights are replicated on every device at engine construction; just record what is loaded"""
@@ -163,6 +163,7 @@ class LocalGPUWorker(Worker):
                 if sampler != "DDIM":
                     logger.warning(f"scheduler '{scheduler}' is not implemented on worker {self.label}: using the sampler's default")
                 scheduler = None
+        controls = self._controls(eng, payload, width, height)
         init_u8 = None
         inpaint = None
         if payload.get("init_images"):
@@ -224,6 +225,8 @@ class LocalGPUWorker(Worker):
         # emphasis multipliers reach the engine only when some weight differs from 1 (all 1 is the unweighted path)
         weighted = lambda m: m is not None and bool((m != 1.0).any())  # noqa: E731
         weights = {"neg_multipliers": neg_mult} if weighted(neg_mult) else {}
+        if controls:   # a payload without ControlNet units reaches the engine with exactly the arguments it always had
+            weights["controls"] = controls
         chunks = []
         for it in range(n_iter):
             # variation seeds: image k of iteration `it` blends noise(seed + k) with noise(subseed + k)
@@ -293,6 +296,19 @@ class LocalGPUWorker(Worker):
                 "parameters": {"batch_size": batch, "n_iter": n_iter, "steps": steps, "width": width, "height": height,
                                "sampler_name": sampler, "cfg_scale": cfg_scale, "seed": seed},
                 "info": json.dumps(info)}
+
+    def _controls(self, eng, payload: dict, width: int, height: int):
+        """the payload's enabled ControlNet units as SDEngine `controls` (None: no unit); refusals raise ValueError"""
+        from b200sd import controlnet as ctl, factory
+        units = ctl.parse_units(payload.get("alwayson_scripts"), width, height)
+        if not units:
+            return None
+        if eng.unet_cfg.adm_in_channels:
+            raise ValueError("ControlNet is not served for SDXL")
+        if payload.get("enable_hr") and not payload.get("init_images"):
+            raise ValueError("ControlNet together with the hires fix is not served")
+        return [(factory.controlnet(u.model, device=str(eng.device), dtype=eng.dtype), u.image, u.weight, u.start, u.end)
+                for u in units]
 
     @staticmethod
     def _init_images_pil(init_images):
