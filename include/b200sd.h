@@ -38,6 +38,7 @@ extern "C" {
 /* epilogue flags for b200sd_linear / b200sd_conv2d */
 #define B200SD_EPI_GEGLU 1 /* tile columns [0,bn/2) = value, [bn/2,bn) = gate: out = v * gelu_erf(g) */
 #define B200SD_EPI_SILU 2  /* out = silu(acc + bias (+ residual)) */
+#define B200SD_EPI_LRELU 4 /* b200sd_conv2d_scaled only: v = leaky_relu(acc + bias, 0.2) */
 
 /* The residual may be the output itself (residual == D and ldr == ldd: D += epi(...) in place, e.g. a ControlNet zero
  * conv adding into a channel slice of a skip-concat buffer): each output tile reads its residual tile before it
@@ -68,6 +69,14 @@ int b200sd_linear(const void* A, long long lda, const void* Wt, void* D, long lo
 int b200sd_conv2d(const void* X, long long pitch_c, int NB, int Hin, int Win, int C, const void* Wt, int ksize,
                   int stride, int pad, int pad_end, void* D, long long ldd, int Cout, int block_n,
                   const b200sd_epilogue* epi, int dtype, int max_ctas, void* stream);
+/* b200sd_conv2d with the epilogue of ESRGAN's RRDBNet (basicsr ResidualDenseBlock / RRDB): v = acc + bias, then
+ * v = leaky_relu(v, 0.2) if epi->flags has B200SD_EPI_LRELU, then D = residual + res_scale * v if epi->residual is set
+ * (else D = v).  epi->flags may hold B200SD_EPI_LRELU only; block_n in {32, 64}; dtype B200SD_F16 only (the upscaler runs
+ * in fp16 for every model family; bf16 returns B200SD_ERR_INVALID).  The residual may equal D as for b200sd_conv2d.
+ * C % 64 == 0. */
+int b200sd_conv2d_scaled(const void* X, long long pitch_c, int NB, int Hin, int Win, int C, const void* Wt, int ksize,
+                         int stride, int pad, int pad_end, void* D, long long ldd, int Cout, int block_n,
+                         const b200sd_epilogue* epi, float res_scale, int dtype, int max_ctas, void* stream);
 
 /* O[b,s,h*d] = softmax(Q K^T * scale) V per (batch, head); Q/K/V rows are tokens, head h occupies columns
  * [h*d_pad, h*d_pad+d) (zero padded to d_pad, a multiple of 64).  (upstream CrossAttention.forward)
@@ -194,6 +203,34 @@ int b200sd_unpack_latent(const void* moments, long long pitch, float* x, int B, 
 /* hires fix, "Latent" upscaler: fp32 NHWC latents [B,H*W,4] -> [B,Ho*Wo,4], bilinear, half-pixel centres, no antialias
  * (torch.nn.functional.interpolate(mode="bilinear") in sdwui StableDiffusionProcessingTxt2Img.sample_hr_pass) */
 int b200sd_resize_latent_bilinear(const float* x, float* y, int B, int H, int W, int Ho, int Wo, void* stream);
+/* hires fix, the other "Latent (...)" upscalers: fp32 NHWC latents [B,H*W,4] -> [B,Ho*Wo,4] by separable DEVICE tables:
+ * y[b,oy,ox] = sum_j wy[oy*ky+j] * (sum_i wx[ox*kx+i] * x[b, iy[oy*ky+j], ix[ox*kx+i]]), sums in tap order.  The host
+ * builds the tables of F.interpolate's nearest, nearest-exact, bicubic (A = -0.75, clamped taps) and antialiased
+ * bilinear / bicubic modes; unused taps carry weight 0 and a valid index. */
+int b200sd_resize_latent_table(const float* x, float* y, int B, int H, int W, int Ho, int Wo, const int* ix,
+                               const float* wx, int kx, const int* iy, const float* wy, int ky, void* stream);
+
+/* ---- hires fix pixel upscalers (sdwui images.resize_image / upscaler_utils.upscale_with_model) ---------------------- */
+/* one pass of Pillow's ImagingResample on RGB uint8 [B,Hin,Win,3] -> [B,Hout,Wout,3] along x (vertical = 0: Hout == Hin)
+ * or y (vertical = 1: Wout == Win).  bounds [out][2] = {first input, count} and kk [out][ksize] are Pillow's fixed-point
+ * coefficients (22 fraction bits), DEVICE arrays; out = clip8((1 << 21 + sum in * kk) >> 22).  Pillow resizes
+ * horizontally first and skips a pass whose size does not change; a NEAREST resize is the same two passes with one
+ * tap of weight 1 << 22 at Pillow's nearest source index. */
+int b200sd_resample_u8(const unsigned char* in, unsigned char* out, int B, int Hin, int Win, int Hout, int Wout,
+                       int vertical, const int* bounds, const int* kk, int ksize, void* stream);
+/* sdwui images.combine_grid: upscaled tiles uint8 [B*rows*cols, th, tw, 3] (row-major per image) -> [B,H,W,3].  Tile (r,c)
+ * sits at (xs[c], ys[r]) (DEVICE arrays, may be negative); within a row each tile not at x == 0 blends its first
+ * `overlap` columns over the row through mask[column] with Pillow's paste-with-mask integer arithmetic, then the rows
+ * are stacked the same way through mask[row]; bitwise equal to the sequence of PIL pastes. */
+int b200sd_combine_tiles_u8(const unsigned char* tiles, unsigned char* out, int B, int H, int W, int th, int tw,
+                            int rows, int cols, const int* ys, const int* xs, const unsigned char* mask, int overlap,
+                            void* stream);
+/* ESRGAN output [B,HW,pitch] (channels 0..2 nominally in [0,1]) -> uint8 [B,HW,3] = round_half_even(255 * clamp(v, 0, 1))
+ * (sdwui torch_bgr_to_pil_image; not the truncating b200sd_quantize_u8 of VAE images).  dtype B200SD_F16 only. */
+int b200sd_quantize_unit_u8(const void* img, long long pitch, unsigned char* out, int B, int HW, int dtype, void* stream);
+/* Y[r, c] += alpha * X[r, c] for c < C, fp32 math (basicsr RRDB: x + 0.2 * rdb3(...)).  dtype B200SD_F16 only. */
+int b200sd_scaled_add(const void* X, long long pitch_x, void* Y, long long pitch_y, long long rows, int C, float alpha,
+                      int dtype, void* stream);
 
 /* inpainting: x[b,p,:] = x[b,p,:] * latmask[p] + init[b,p,:] * (1 - latmask[p]) on fp32 NHWC latents [B,HW,4]; latmask [HW]
  * is the request's latent-resolution mask (1 = repaint).  (sdwui CFGDenoiser.apply_blend, before every model call of the

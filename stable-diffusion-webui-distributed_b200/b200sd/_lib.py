@@ -24,6 +24,7 @@ class Epilogue(ctypes.Structure):
 
 EPI_GEGLU = 1
 EPI_SILU = 2
+EPI_LRELU = 4
 F16 = 0
 BF16 = 1
 

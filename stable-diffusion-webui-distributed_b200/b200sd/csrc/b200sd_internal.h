@@ -10,7 +10,7 @@ int gemm_tc(const void* A, long long lda, const void* Wt, void* D, long long ldd
 
 int conv_tc(const void* X, long long pitch_c, int NB, int Hin, int Win, int C, const void* Wt, int ksize, int stride,
             int pad, int pad_end, void* D, long long ldd, int Cout, int block_n, const b200sd_epilogue* epi,
-            int is_bf16, int max_ctas, cudaStream_t stream);
+            int is_bf16, int max_ctas, cudaStream_t stream, bool scaled = false, float res_scale = 1.0f);
 
 int attention_tc(const void* Q, long long ldq, const void* K, long long ldk, const void* V, long long ldv, void* O,
                  long long ldo, int B, int heads, int Sq, int Skv, const int* kv_len, int d, int d_pad, float scale,

@@ -59,6 +59,7 @@ struct GemmKernelParams {
   int bias_group_rows;             // rows (output pixels) sharing one bias row; <= 0 -> single row
   int has_residual;
   int flags;                       // B200SD_EPI_*
+  float res_scale;                 // b200sd_conv2d_scaled only: D = residual + res_scale * v
 };
 
 struct __align__(8) GemmBarriers {
@@ -151,11 +152,13 @@ __device__ __forceinline__ void load_residual(const GemmKernelParams& p, const C
   else tma_load_4d(dst, tmR, &bars->res_full[buf], col, tc.c1, tc.c2, tc.c3);
 }
 
-template <int BN, bool kBf16>
-__global__ void __launch_bounds__(kGemmThreads, 1)
-gemm_conv_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
-                    const __grid_constant__ CUtensorMap tmD, const __grid_constant__ CUtensorMap tmR,
-                    const GemmKernelParams p) {
+// kScaled = false: the b200sd_linear / b200sd_conv2d epilogue (+bias, GEGLU, +residual, SiLU).
+// kScaled = true:  the b200sd_conv2d_scaled epilogue (+bias, LeakyReLU(0.2), D = residual + res_scale * v), ESRGAN's
+//                  RRDBNet convolutions; a separate instantiation, so the kernels above keep their code.
+template <int BN, bool kBf16, bool kScaled>
+__device__ __forceinline__ void gemm_conv_tc_body(const CUtensorMap& tmA, const CUtensorMap& tmB,
+                                                  const CUtensorMap& tmD, const CUtensorMap& tmR,
+                                                  const GemmKernelParams p) {
   constexpr uint32_t kStageBytes = kATileBytes + BN * 128u;
   extern __shared__ uint8_t smem_raw[];
   // SWIZZLE_128B tiles need 1024-byte alignment.
@@ -308,6 +311,9 @@ gemm_conv_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_consta
                 constexpr int kGate = BN / 4;  // accumulator index distance of column + BN/2
                 v *= gelu_erf(acc[(idx + kGate) % (BN / 2)] + (e ? bg.y : bg.x));
               }
+              if constexpr (kScaled) {
+                if (p.flags & B200SD_EPI_LRELU) v = v > 0.f ? v : v * 0.2f;
+              }
               f[h][g][e] = v;
             }
           }
@@ -322,11 +328,16 @@ gemm_conv_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_consta
 #pragma unroll
             for (int g = 0; g < 4; ++g) {
               const float2 t = unpack2<kBf16>(*reinterpret_cast<const uint32_t*>(rt + sw64_offset(row0 + 8 * h, g) + colq * 2));
-              f[h][g][0] += t.x;
-              f[h][g][1] += t.y;
+              if constexpr (kScaled) {
+                f[h][g][0] = __fmaf_rn(p.res_scale, f[h][g][0], t.x);
+                f[h][g][1] = __fmaf_rn(p.res_scale, f[h][g][1], t.y);
+              } else {
+                f[h][g][0] += t.x;
+                f[h][g][1] += t.y;
+              }
             }
         }
-        if (p.flags & B200SD_EPI_SILU) {
+        if (!kScaled && (p.flags & B200SD_EPI_SILU)) {
 #pragma unroll
           for (int h = 0; h < 2; ++h)
 #pragma unroll
@@ -358,10 +369,35 @@ gemm_conv_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_consta
   if (leader) bulk_wait<0>();  // the TMA stores must have completed before the CTA (and its smem) goes away
 }
 
+template <int BN, bool kBf16>
+__global__ void __launch_bounds__(kGemmThreads, 1)
+gemm_conv_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
+                    const __grid_constant__ CUtensorMap tmD, const __grid_constant__ CUtensorMap tmR,
+                    const GemmKernelParams p) {
+  gemm_conv_tc_body<BN, kBf16, false>(tmA, tmB, tmD, tmR, p);
+}
+
+template <int BN, bool kBf16>
+__global__ void __launch_bounds__(kGemmThreads, 1)
+conv_scaled_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
+                      const __grid_constant__ CUtensorMap tmD, const __grid_constant__ CUtensorMap tmR,
+                      const GemmKernelParams p) {
+  gemm_conv_tc_body<BN, kBf16, true>(tmA, tmB, tmD, tmR, p);
+}
+
 // ------------------------------------------------------------------------------------------------
 // host side
 // ------------------------------------------------------------------------------------------------
 typedef void (*GemmKernel)(CUtensorMap, CUtensorMap, CUtensorMap, CUtensorMap, GemmKernelParams);
+
+// the scaled-epilogue convolutions of RRDBNet: fp16 (the upscaler's precision for every model family), 32 (dense-block
+// growth) or 64 output channels per tile
+static GemmKernel scaled_kernel_for(int block_n, int is_bf16) {
+  if (is_bf16) return nullptr;
+  if (block_n == 32) return conv_scaled_tc_kernel<32, false>;
+  if (block_n == 64) return conv_scaled_tc_kernel<64, false>;
+  return nullptr;
+}
 
 template <bool kBf16>
 static GemmKernel kernel_for(int block_n) {
@@ -397,8 +433,9 @@ static int device_props() {
       return B200SD_ERR_CUDA;
     for (int bn = 32; bn <= 256; bn += 32)
       for (int bf = 0; bf < 2; ++bf)
-        if (cudaFuncSetAttribute(kernel_for(bn, bf), cudaFuncAttributeMaxDynamicSharedMemorySize, smem) != cudaSuccess)
-          return B200SD_ERR_CUDA;
+        for (GemmKernel k : {kernel_for(bn, bf), scaled_kernel_for(bn, bf)})
+          if (k != nullptr && cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, smem) != cudaSuccess)
+            return B200SD_ERR_CUDA;
     g_num_sms = sms;
     g_max_smem = smem;
     g_dev_ready[dev] = true;
@@ -407,7 +444,7 @@ static int device_props() {
 }
 
 static int launch(const CUtensorMap& tmA, const CUtensorMap& tmB, const CUtensorMap& tmD, const CUtensorMap& tmR,
-                  GemmKernelParams& p, int is_bf16, int max_ctas, cudaStream_t stream) {
+                  GemmKernelParams& p, int is_bf16, int max_ctas, cudaStream_t stream, bool scaled = false) {
   const uint32_t stage_bytes = kATileBytes + static_cast<uint32_t>(p.block_n) * 128u;
   const int staging = (p.has_residual ? 4 : 2) * static_cast<int>(kStageTileBytes);
   const int budget = g_max_smem - 1024 /*align*/ - staging - static_cast<int>(sizeof(GemmBarriers));
@@ -420,7 +457,7 @@ static int launch(const CUtensorMap& tmA, const CUtensorMap& tmB, const CUtensor
   int grid = num_tiles < g_num_sms ? num_tiles : g_num_sms;
   if (max_ctas > 0 && grid > max_ctas) grid = max_ctas;
   if (grid <= 0) return B200SD_OK;
-  GemmKernel k = kernel_for(p.block_n, is_bf16);
+  GemmKernel k = scaled ? scaled_kernel_for(p.block_n, is_bf16) : kernel_for(p.block_n, is_bf16);
   if (k == nullptr) return B200SD_ERR_INVALID;
   launch_pdl(k, dim3(grid), dim3(kGemmThreads), smem, stream, tmA, tmB, tmD, tmR, p);
   return cudaGetLastError() == cudaSuccess ? B200SD_OK : B200SD_ERR_CUDA;
@@ -528,9 +565,10 @@ int gemm_tc(const void* A, long long lda, const void* Wt, void* D, long long ldd
 
 int conv_tc(const void* X, long long pitch_c, int NB, int Hin, int Win, int C, const void* Wt, int ksize, int stride,
             int pad, int pad_end, void* D, long long ldd, int Cout, int block_n, const b200sd_epilogue* epi,
-            int is_bf16, int max_ctas, cudaStream_t stream) {
+            int is_bf16, int max_ctas, cudaStream_t stream, bool scaled, float res_scale) {
   if (NB <= 0) return B200SD_OK;
   if ((ksize != 3 && ksize != 1) || (stride != 1 && stride != 2) || C % kBlockK != 0) return B200SD_ERR_INVALID;
+  if (scaled && epi != nullptr && (epi->flags & ~B200SD_EPI_LRELU) != 0) return B200SD_ERR_INVALID;
   if (pitch_c % 8 != 0 || (reinterpret_cast<uintptr_t>(X) & 15) != 0 || (reinterpret_cast<uintptr_t>(Wt) & 15) != 0)
     return B200SD_ERR_INVALID;
   const int taps = ksize * ksize;
@@ -543,6 +581,7 @@ int conv_tc(const void* X, long long pitch_c, int NB, int Hin, int Win, int C, c
   int rc = fill_common(p, o, NB * Ho * Wo, Cout, taps * C, block_n, epi, D, ldd, is_bf16);
   if (rc != B200SD_OK) return rc;
   p.mode = 1;
+  p.res_scale = res_scale;
   p.H = Ho; p.W = Wo; p.NB = NB;
   p.taps = taps; p.cblocks = C / kBlockK; p.stride = stride; p.pad = pad;
   // output-pixel box: as much of a row as fits, then rows, then images (all <= 128 pixels)
@@ -582,7 +621,7 @@ int conv_tc(const void* X, long long pitch_c, int NB, int Hin, int Win, int C, c
   }
   rc = make_out_maps(p, o, &tmD, &tmR);
   if (rc != B200SD_OK) return rc;
-  return launch(tmA, tmB, tmD, tmR, p, is_bf16, max_ctas, stream);
+  return launch(tmA, tmB, tmD, tmR, p, is_bf16, max_ctas, stream, scaled);
 }
 
 }  // namespace b200sd

@@ -915,20 +915,38 @@ class SDEngine:
                       cfg_scale: float = 7.0, height: int = 512, width: int = 512, hr_scale: float = 2.0,
                       hr_steps: int = 0, denoising_strength: float = 0.7, sampler: str = "DDIM",
                       scheduler: Optional[str] = None, multipliers: Optional[torch.Tensor] = None,
-                      neg_multipliers: Optional[torch.Tensor] = None) -> torch.Tensor:
-        """txt2img with sdwui's hires fix and the "Latent" upscaler (StableDiffusionProcessingTxt2Img.sample /
-        sample_hr_pass): first pass at (height, width), bilinear resize of the latents to hr_scale x, a fresh per-image
-        noise of the large shape from the same seeds, then the same sampler's img2img half from t_enc with `hr_steps`
-        (0 = `steps`) steps, decode at the large size.  Returns uint8 [b, H*hr, W*hr, 3] on device."""
+                      neg_multipliers: Optional[torch.Tensor] = None, upscaler: str = "Latent",
+                      upscaler_tile: int = 192, upscaler_overlap: int = 8) -> torch.Tensor:
+        """txt2img with sdwui's hires fix (StableDiffusionProcessingTxt2Img.sample / sample_hr_pass): first pass at
+        (height, width), the `upscaler` to hr_scale x, a fresh per-image noise of the large shape from the same seeds,
+        then the same sampler's img2img half from t_enc with `hr_steps` (0 = `steps`) steps, decode at the large size.
+        `upscaler` (b200sd.upscale): a "Latent ..." mode resizes the latents (F.interpolate); any other name decodes the
+        first pass, resizes the uint8 images as sdwui's images.resize_image does (ESRGAN tiles of `upscaler_tile` pixels
+        overlapping by `upscaler_overlap`) and VAE-encodes the result as img2img encodes init images.
+        Returns uint8 [b, H*hr, W*hr, 3] on device."""
+        from . import upscale
+        kind, _ = upscale.kind(upscaler)
         b = tokens.shape[0]
         h, w = height // 8, width // 8
         h2, w2 = int(height * hr_scale) // 8, int(width * hr_scale) // 8
+        if kind != "latent" and (int(height * hr_scale) % 8 or int(width * hr_scale) % 8):
+            raise ValueError(f"hires upscaler {upscaler!r}: the target size must be a multiple of 8")
         cond, uncond = self._conds(tokens, neg_tokens, width, height, multipliers, neg_multipliers)
         lat = self._sample_txt(cond, uncond, seed, b, h, w, steps, cfg_scale, sampler, scheduler)
-        with self._ctx():
-            up = torch.empty((b, h2 * w2, 4), device=self.device, dtype=torch.float32)
-            ops.resize_latent_bilinear(lat.contiguous(), up, h, w, h2, w2)
-        init = up.reshape(b, h2, w2, 4).permute(0, 3, 1, 2)
+        if kind == "latent":
+            with self._ctx():
+                if upscaler == "Latent":
+                    up = torch.empty((b, h2 * w2, 4), device=self.device, dtype=torch.float32)
+                    ops.resize_latent_bilinear(lat.contiguous(), up, h, w, h2, w2)
+                else:
+                    up = upscale.resize_latents(lat, upscaler, h, w, h2, w2)
+            init = up.reshape(b, h2, w2, 4).permute(0, 3, 1, 2)
+        else:
+            images = self.decode(lat, h, w)
+            f = 2 ** (len(self.vae_cfg.ch_mult) - 1)   # 8 for the kl-f8 autoencoder: the target is then W*hr x H*hr
+            with self._ctx():
+                images = upscale.resize_image(images, w2 * f, h2 * f, upscaler, upscaler_tile, upscaler_overlap)
+            init = self.encode(images.contiguous())
         if self.clip.xl:   # SDXL's vector conditioning carries the target size: the second pass gets its own (sdwui hr_c / hr_uc)
             cond, uncond = self._conds(tokens, neg_tokens, w2 * 8, h2 * 8, multipliers, neg_multipliers)
         lat2 = self._sample_from(init, cond, uncond, seed, denoising_strength, hr_steps or steps, cfg_scale, sampler, scheduler)

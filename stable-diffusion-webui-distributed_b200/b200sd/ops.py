@@ -10,7 +10,7 @@ from typing import Optional
 import torch
 
 from . import _lib
-from ._lib import BF16, EPI_GEGLU, EPI_SILU, F16, Epilogue, check
+from ._lib import BF16, EPI_GEGLU, EPI_LRELU, EPI_SILU, F16, Epilogue, check
 
 LAUNCHES = 0  # number of b200sd kernels launched through this module (bench.py's gpu_launches)
 
@@ -430,3 +430,93 @@ def bump_step(step_counter: torch.Tensor):
     rc = _lib.lib().b200sd_bump_step(_p(step_counter), _stream())
     check(rc, "b200sd_bump_step")
     _count()
+
+
+# ---- hires fix upscalers (b200sd/upscale.py builds the tables these take)
+def conv2d_scaled(x: torch.Tensor, wt: torch.Tensor, out: torch.Tensor, bias: Optional[torch.Tensor] = None,
+                  residual: Optional[torch.Tensor] = None, res_scale: float = 1.0, lrelu: bool = False,
+                  block_n: Optional[int] = None, max_ctas: int = 0):
+    """3x3 / pad 1 conv with the RRDBNet epilogue: v = acc + bias, LeakyReLU(0.2) if `lrelu`, then
+    out = residual + res_scale * v when a residual is given.  x [NB, H, W, C] NHWC (channel pitch x.stride(2))."""
+    nb, h, w, c = x.shape
+    assert x.stride(3) == 1 and x.stride(1) == w * x.stride(2) and x.stride(0) == h * x.stride(1)
+    cout, kk = wt.shape
+    assert kk == 9 * c and wt.is_contiguous()
+    mo, no, ldd = _rows2d(out)
+    bn = block_n or (64 if cout % 64 == 0 else 32)
+    e = _epi(bias, 0, residual, EPI_LRELU if lrelu else 0)
+    rc = _lib.lib().b200sd_conv2d_scaled(_p(x), ctypes.c_longlong(x.stride(2)), nb, h, w, c, _p(wt), 3, 1, 1, 1,
+                                         _p(out), ctypes.c_longlong(ldd), cout, bn, ctypes.byref(e),
+                                         ctypes.c_float(res_scale), _dt(x), max_ctas, _stream())
+    check(rc, f"b200sd_conv2d_scaled NB={nb} H={h} W={w} C={c} Cout={cout}")
+    _count()
+    return out
+
+
+def resample_u8(x: torch.Tensor, out: torch.Tensor, vertical: bool, bounds: torch.Tensor, kk: torch.Tensor):
+    """one Pillow resampling pass, uint8 [B, H, W, 3] -> [B, Ho, Wo, 3]; bounds int32 [n, 2], kk int32 [n, ksize] on the
+    device"""
+    b, hi, wi, _ = x.shape
+    _, ho, wo, _ = out.shape
+    assert x.dtype == out.dtype == torch.uint8 and x.is_contiguous() and out.is_contiguous()
+    assert bounds.dtype == kk.dtype == torch.int32 and bounds.is_contiguous() and kk.is_contiguous()
+    assert bounds.shape == ((ho if vertical else wo), 2) and kk.shape[0] == bounds.shape[0]
+    rc = _lib.lib().b200sd_resample_u8(_p(x), _p(out), b, hi, wi, ho, wo, int(vertical), _p(bounds), _p(kk),
+                                       kk.shape[1], _stream())
+    check(rc, "b200sd_resample_u8")
+    _count()
+    return out
+
+
+def combine_tiles_u8(tiles: torch.Tensor, out: torch.Tensor, ys: torch.Tensor, xs: torch.Tensor, mask: torch.Tensor,
+                     overlap: int):
+    """tiles uint8 [B * rows * cols, th, tw, 3] -> out uint8 [B, H, W, 3] (sdwui combine_grid); ys/xs int32, mask uint8
+    [overlap] on the device"""
+    b, hh, ww, _ = out.shape
+    _, th, tw, _ = tiles.shape
+    rows, cols = ys.numel(), xs.numel()
+    assert tiles.shape[0] == b * rows * cols and tiles.dtype == out.dtype == mask.dtype == torch.uint8
+    assert tiles.is_contiguous() and out.is_contiguous() and ys.dtype == xs.dtype == torch.int32
+    rc = _lib.lib().b200sd_combine_tiles_u8(_p(tiles), _p(out), b, hh, ww, th, tw, rows, cols, _p(ys), _p(xs), _p(mask),
+                                            overlap, _stream())
+    check(rc, "b200sd_combine_tiles_u8")
+    _count()
+    return out
+
+
+def quantize_unit_u8(img: torch.Tensor, out: torch.Tensor):
+    """img [B, HW, pitch>=3] -> out uint8 [B, HW, 3] = round(255 * clamp(v, 0, 1))"""
+    b, hw, _ = img.shape
+    assert out.dtype == torch.uint8 and out.is_contiguous() and img.stride(2) == 1 and img.stride(0) == hw * img.stride(1)
+    rc = _lib.lib().b200sd_quantize_unit_u8(_p(img), ctypes.c_longlong(img.stride(1)), _p(out), b, hw, _dt(img),
+                                            _stream())
+    check(rc, "b200sd_quantize_unit_u8")
+    _count()
+    return out
+
+
+def scaled_add_(y: torch.Tensor, x: torch.Tensor, alpha: float):
+    """y += alpha * x over [rows, C] (row pitches from stride(-2)), in place"""
+    rows, c, ldy = _rows2d(y)
+    rx, cx, ldx = _rows2d(x)
+    assert (rx, cx) == (rows, c) and x.dtype == y.dtype
+    rc = _lib.lib().b200sd_scaled_add(_p(x), ctypes.c_longlong(ldx), _p(y), ctypes.c_longlong(ldy),
+                                      ctypes.c_longlong(rows), c, ctypes.c_float(alpha), _dt(y), _stream())
+    check(rc, "b200sd_scaled_add")
+    _count()
+    return y
+
+
+def resize_latent_table(x: torch.Tensor, y: torch.Tensor, h: int, w: int, ho: int, wo: int, tx, ty):
+    """x fp32 [B, h*w, 4] -> y fp32 [B, ho*wo, 4] by the separable tables tx = (ix int32 [wo, kx], wx fp32 [wo, kx]) and
+    ty = (iy [ho, ky], wy [ho, ky]) on the device"""
+    b = x.shape[0]
+    assert x.dtype == torch.float32 and y.dtype == torch.float32 and x.is_contiguous() and y.is_contiguous()
+    assert x.shape == (b, h * w, 4) and y.shape == (b, ho * wo, 4)
+    (ix, wx), (iy, wy) = tx, ty
+    assert ix.shape == wx.shape and ix.shape[0] == wo and iy.shape == wy.shape and iy.shape[0] == ho
+    rc = _lib.lib().b200sd_resize_latent_table(_p(x), _p(y), b, h, w, ho, wo, _p(ix), _p(wx), ix.shape[1], _p(iy),
+                                               _p(wy), iy.shape[1], _stream())
+    check(rc, "b200sd_resize_latent_table")
+    _count()
+    return y

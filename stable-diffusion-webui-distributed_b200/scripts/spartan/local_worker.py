@@ -87,8 +87,9 @@ class LocalGPUWorker(Worker):
     def restart(self) -> bool:
         """reference Worker.restart posts /server-restart; here: drop the engine (weights, plans, graphs) — the next
         request rebuilds it"""
-        from b200sd import factory
+        from b200sd import factory, upscale
         factory.evict(self.device)
+        upscale.evict(self.device)
         self._engine = None
         return True
 
@@ -241,18 +242,17 @@ class LocalGPUWorker(Worker):
                 u8 = eng.img2img(tok, neg_all, seed_it, init_u8, denoising_strength=denoise, steps=steps,
                                  cfg_scale=cfg_scale, sampler=sampler, scheduler=scheduler, **kw, **weights)
             elif payload.get("enable_hr"):
-                # hires fix (reference eta_hr, worker.py:205): second pass at hr_scale x with the "Latent" upscaler
-                upscaler = payload.get("hr_upscaler") or "Latent"
-                if upscaler != "Latent":
-                    logger.warning(f"hires upscaler '{upscaler}' is not implemented on worker {self.label}: using 'Latent'")
+                # hires fix (reference eta_hr, worker.py:205): second pass at hr_scale x after the hr_upscaler
                 hr_scale = float(payload.get("hr_scale") or 2.0)
                 if payload.get("hr_resize_x") and payload.get("hr_resize_y"):
                     hr_scale = float(payload["hr_resize_x"]) / width
+                hires = dict(weights)
+                hires.update(self._hires_upscaler(payload, width, height, hr_scale))
                 u8 = eng.txt2img_hires(tok, neg_all, seed_it, steps=steps, cfg_scale=cfg_scale, height=height,
                                        width=width, hr_scale=hr_scale,
                                        hr_steps=int(payload.get("hr_second_pass_steps") or 0),
                                        denoising_strength=0.7 if ds is None else float(ds), sampler=sampler,
-                                       scheduler=scheduler, **weights)
+                                       scheduler=scheduler, **hires)
             else:
                 u8 = eng.txt2img(tok, neg_all, seed_it, steps=steps, cfg_scale=cfg_scale, height=height,
                                  width=width, sampler=sampler, scheduler=scheduler, **weights)
@@ -296,6 +296,32 @@ class LocalGPUWorker(Worker):
                 "parameters": {"batch_size": batch, "n_iter": n_iter, "steps": steps, "width": width, "height": height,
                                "sampler_name": sampler, "cfg_scale": cfg_scale, "seed": seed},
                 "info": json.dumps(info)}
+
+    def _hires_upscaler(self, payload: dict, width: int, height: int, hr_scale: float) -> dict:
+        """txt2img_hires keyword arguments for the payload's hr_upscaler: none for "Latent" (the call keeps exactly its
+        arguments), else the upscaler and, for ESRGAN models, sdwui's ESRGAN_tile / ESRGAN_tile_overlap settings.
+        An upscaler that is not served falls back to "Latent" with a warning."""
+        from b200sd import upscale
+        name = payload.get("hr_upscaler") or "Latent"
+        if name == "Latent":
+            return {}
+        try:
+            kind, stem = upscale.kind(name)
+            if kind != "latent" and (int(width * hr_scale) % 8 or int(height * hr_scale) % 8):
+                raise upscale.UnsupportedUpscaler("the hires size is not a multiple of 8")
+            if kind == "esrgan":   # load (and cache) the model now: a file that is not a 4x RRDBNet falls back
+                upscale.model(stem, self.engine.device)
+        except upscale.UnsupportedUpscaler as e:
+            logger.warning(f"hires upscaler '{name}' is not implemented on worker {self.label} ({e}): using 'Latent'")
+            return {}
+        out = {"upscaler": name}
+        if kind == "esrgan":
+            opts = payload.get("override_settings") or {}
+            if opts.get("ESRGAN_tile") is not None:
+                out["upscaler_tile"] = int(opts["ESRGAN_tile"])
+            if opts.get("ESRGAN_tile_overlap") is not None:
+                out["upscaler_overlap"] = int(opts["ESRGAN_tile_overlap"])
+        return out
 
     def _controls(self, eng, payload: dict, width: int, height: int):
         """the payload's enabled ControlNet units as SDEngine `controls` (None: no unit); refusals raise ValueError"""
