@@ -120,6 +120,13 @@ int b200sd_layernorm(const void* X, long long ldx, void* Y, long long ldy, int r
 /* nearest-neighbour 2x upsample, NHWC. (upstream Upsample before its conv) */
 int b200sd_upsample2x(const void* X, long long pitch_x, void* Y, long long pitch_y, int NB, int H, int W, int C,
                       int dtype, void* stream);
+/* circular padding, NHWC: X[NB,H,W,C] (pixel pitch pitch_x) -> Y[NB,H+2p,W+2p,C] (pixel pitch pitch_y), the interior X and
+ * the halo copied from the opposite edges, as torch.nn.functional.pad(mode="circular").  A pure copy: the output is
+ * bitwise defined.  0 <= p <= H and p <= W (H = 1 or W = 1 with p = 1 wraps onto itself); C % 8 == 0.  A circular 3x3
+ * conv (sdwui's tiling: padding_mode 'circular' on every Conv2d) is this copy with p = 1, then b200sd_conv2d with
+ * pad = pad_end = 0 on Y. */
+int b200sd_pad_circular(const void* X, long long pitch_x, void* Y, long long pitch_y, int NB, int H, int W, int C, int p,
+                        int dtype, void* stream);
 /* row softmax of an fp16/bf16 matrix in place, fp32 math (VAE mid-block attention, d=512 single head). */
 int b200sd_softmax_rows(void* S, long long lds, int rows, int cols, float scale, int dtype, void* stream);
 /* Y[rows, C] = silu(X) elementwise (emb_layers SiLU). */

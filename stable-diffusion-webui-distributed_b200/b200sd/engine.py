@@ -259,15 +259,16 @@ class Program:
 
 # ------------------------------------------------------------------------------------------------ plans
 class Plan:
-    """Everything shape-dependent for (images per call b, latent h x w) on one device."""
+    """Everything shape-dependent for (images per call b, latent h x w) on one device.  tiling: the UNet's and the VAE
+    decoder's 3x3 convs pad circularly (sdwui's tiling option)."""
 
-    def __init__(self, eng: "SDEngine", b: int, h: int, w: int, vae_chunk: int):
+    def __init__(self, eng: "SDEngine", b: int, h: int, w: int, vae_chunk: int, tiling: bool = False):
         dev = eng.device
         self.b, self.h, self.w = b, h, w
-        self.unet = UNetProgram(eng.unet_w, 2 * b, h, w, CHUNK)
+        self.unet = UNetProgram(eng.unet_w, 2 * b, h, w, CHUNK, tiling=tiling)
         self.kv_len = self.unet.kv_len   # int32 [2b] on the device: context tokens of every [cond | uncond] row
         self.vae_chunk = min(vae_chunk, b)
-        self.vae = VAEDecoderProgram(eng.vae_w, self.vae_chunk, h, w)
+        self.vae = VAEDecoderProgram(eng.vae_w, self.vae_chunk, h, w, tiling=tiling)
         self.x = torch.zeros((b, h * w, 4), device=dev, dtype=torch.float32)
         self.step = torch.zeros((1,), device=dev, dtype=torch.int32)
         self.coef = torch.zeros((MAX_STEPS, 4), device=dev, dtype=torch.float32)
@@ -444,8 +445,9 @@ class SDEngine:
             self._cap_stream = torch.cuda.Stream(device=self.device)
         return self._cap_stream
 
-    def plan(self, b: int, h: int, w: int) -> Plan:
-        key = (b, h, w)
+    def plan(self, b: int, h: int, w: int, tiling: bool = False) -> Plan:
+        """the plan of (b, h, w); tiled plans are kept apart under (b, h, w, "tiling")"""
+        key = (b, h, w, "tiling") if tiling else (b, h, w)
         down = 2 ** (len(self.unet_cfg.channel_mult) - 1)
         if b < 1 or h < down or w < down or h % down or w % down:
             # the UNet halves the latent len(channel_mult) - 1 times and concatenates skip tensors on the way up: upstream
@@ -457,7 +459,7 @@ class SDEngine:
                 old = self.plans.pop(next(iter(self.plans)))
                 old.graphs.clear()
             with self._ctx():
-                self.plans[key] = Plan(self, b, h, w, self.vae_chunk)
+                self.plans[key] = Plan(self, b, h, w, self.vae_chunk, tiling)
         else:
             self.plans[key] = self.plans.pop(key)   # most recently used last
         return self.plans[key]
@@ -633,11 +635,13 @@ class SDEngine:
 
     @torch.no_grad()
     def run_program(self, cond: torch.Tensor, uncond: torch.Tensor, x_start: torch.Tensor, pr: "Program", cfg_scale: float,
-                    noises: Optional[torch.Tensor] = None, inpaint=None, controls=None) -> torch.Tensor:
+                    noises: Optional[torch.Tensor] = None, inpaint=None, controls=None,
+                    tiling: bool = False) -> torch.Tensor:
         """cond/uncond [b, 77 * k, ctx] on device (cond and uncond may have different k); x_start [b, 4, h, w] fp32 (host or device) = Program.start(...): the start
         latents in the sampler's own space; noises [pr.draws, b, 4, h, w]: the per-image N(0,1) draws after the first;
         inpaint = (clean init latents [b, 4, h, w], latent mask [h * w]).  controls: ControlNet units, see _set_controls
-        (None: no ControlNet).  Returns the final latents fp32 [b, h*w, 4] (NHWC, a view of plan state)."""
+        (None: no ControlNet).  tiling: the UNet's convs pad circularly (its own plan).  Returns the final latents fp32
+        [b, h*w, 4] (NHWC, a view of plan state)."""
         b, _, h, w = x_start.shape
         if pr.draws and (noises is None or noises.shape[0] < pr.draws):
             raise ValueError(f"{pr.sampler} needs {pr.draws} per-image noise draws")
@@ -647,7 +651,7 @@ class SDEngine:
         cond = cond if isinstance(cond, Cond) else Cond(cond)
         uncond = uncond if isinstance(uncond, Cond) else Cond(uncond)
         with self._ctx():
-            plan = self.plan(b, h, w)
+            plan = self.plan(b, h, w, tiling)
             if controls and cond.y is not None:
                 raise ValueError("ControlNet is not served for SDXL")
             self._windows = self._set_controls(plan, controls) if controls else []
@@ -812,11 +816,12 @@ class SDEngine:
         return self.run_program(cond, uncond, x_T.to(torch.float32) * pr.noise_scale, pr, cfg_scale, noises, inpaint)
 
     @torch.no_grad()
-    def decode(self, latents: torch.Tensor, h: int, w: int) -> torch.Tensor:
-        """latents fp32 [b, h*w, 4] (scaled) -> uint8 [b, 8h, 8w, 3] on device."""
+    def decode(self, latents: torch.Tensor, h: int, w: int, tiling: bool = False) -> torch.Tensor:
+        """latents fp32 [b, h*w, 4] (scaled) -> uint8 [b, 8h, 8w, 3] on device.  tiling: circular convs (the tiled plan's
+        decoder)."""
         b = latents.shape[0]
         with self._ctx():
-            plan = self.plan(b, h, w)
+            plan = self.plan(b, h, w, tiling)
             vae = plan.vae
             out = torch.empty((b, vae.out_h * vae.out_w, 3), device=self.device, dtype=torch.uint8)
             c = plan.vae_chunk
@@ -845,17 +850,17 @@ class SDEngine:
             return out.reshape(b, vae.out_h, vae.out_w, 3)
 
     @torch.no_grad()
-    def encode(self, images_u8: torch.Tensor) -> torch.Tensor:
+    def encode(self, images_u8: torch.Tensor, tiling: bool = False) -> torch.Tensor:
         """images uint8 [b, H, W, 3] (host or device) -> scaled latents fp32 [b, 4, H/f, W/f] (posterior mean), in
-        chunks of `vae_chunk` images."""
+        chunks of `vae_chunk` images.  tiling: circular convs (an encoder program of its own)."""
         b, hh, ww, _ = images_u8.shape
         with self._ctx():
             c = min(self.vae_chunk, b)
-            key = (c, hh, ww)
+            key = (c, hh, ww, "tiling") if tiling else (c, hh, ww)
             if key not in self.encoders:
                 while len(self.encoders) >= MAX_PLANS:
                     self.encoders.pop(next(iter(self.encoders)))
-                self.encoders[key] = VAEEncoderProgram(self.vae_enc_w, c, hh, ww)
+                self.encoders[key] = VAEEncoderProgram(self.vae_enc_w, c, hh, ww, tiling=tiling)
             enc = self.encoders[key]
             imgs = images_u8.to(self.device).reshape(b, hh * ww, 3)
             out = torch.empty((b, enc.lat_h * enc.lat_w, 4), device=self.device, dtype=torch.float32)
@@ -874,7 +879,7 @@ class SDEngine:
                 denoising_strength: float = 0.75, steps: int = 20, cfg_scale: float = 7.0, sampler: str = "DDIM",
                 scheduler: Optional[str] = None, latmask: Optional[torch.Tensor] = None,
                 inpainting_fill: int = 1, multipliers: Optional[torch.Tensor] = None,
-                neg_multipliers: Optional[torch.Tensor] = None, controls=None) -> torch.Tensor:
+                neg_multipliers: Optional[torch.Tensor] = None, controls=None, tiling: bool = False) -> torch.Tensor:
         """img2img: VAE-encode the init images (posterior mean), noise them to t_enc, run the remaining part of the
         sampler's schedule, decode.  init_u8 uint8 [b, H, W, 3].  Returns uint8 [b, H, W, 3] on device.
         `latmask` fp32 [h * w] (b200sd.inpaint.prepare_mask): inpainting — the region with latmask 0 is held to the init
@@ -885,10 +890,12 @@ class SDEngine:
         the request's start noise / by zeros first (sdwui Img2Img.init); 0 ("fill") is image-space work the caller does
         before the call (inpaint.fill_masked), 1 keeps the original content.
         `controls`: ControlNet units [(ControlNetWeights, control map uint8 [H, W, 3], weight, guidance_start,
-        guidance_end)], at most 3 (None: none)."""
+        guidance_end)], at most 3 (None: none).
+        `tiling`: sdwui's tiling option — every 3x3 conv of the UNet and the VAE pads circularly (ControlNet's do
+        not)."""
         b = tokens.shape[0]
         cond, uncond = self._conds(tokens, neg_tokens, init_u8.shape[2], init_u8.shape[1], multipliers, neg_multipliers)
-        init = self.encode(init_u8)
+        init = self.encode(init_u8, tiling)
         _, _, h, w = init.shape
         if latmask is not None and inpainting_fill in (2, 3):
             nm = latmask.to(self.device, torch.float32).reshape(1, 1, h, w)
@@ -896,11 +903,12 @@ class SDEngine:
             if inpainting_fill == 2:   # create_random_tensors(shape, seeds): the same first draw the sampler starts from
                 init = init + per_image_noise(seed, b, (4, h, w), 1, *self.variation)[0].to(self.device) * nm
         lat = self._sample_from(init, cond, uncond, seed, denoising_strength, steps, cfg_scale, sampler, scheduler,
-                                inpaint=None if latmask is None else (init, latmask), controls=controls)
-        return self.decode(lat, h, w)
+                                inpaint=None if latmask is None else (init, latmask), controls=controls, tiling=tiling)
+        return self.decode(lat, h, w, tiling)
 
     def _sample_from(self, init: torch.Tensor, cond, uncond, seed: int, denoising_strength: float, steps: int,
-                     cfg_scale: float, sampler: str, scheduler: Optional[str], inpaint=None, controls=None) -> torch.Tensor:
+                     cfg_scale: float, sampler: str, scheduler: Optional[str], inpaint=None, controls=None,
+                     tiling: bool = False) -> torch.Tensor:
         """the img2img half of a sampler (also the second pass of the hires fix): `init` [b, 4, h, w] latents on the device,
         fresh per-image noise from `seed`, start at the noise level of t_enc.
         DDIM / PLMS: sdwui sd_samplers_timesteps.sample_img2img; k-diffusion samplers: KDiffusionSampler.sample_img2img."""
@@ -908,7 +916,7 @@ class SDEngine:
         pr = self.program(sampler, scheduler, steps, denoise=denoising_strength, masked=inpaint is not None)
         nz = per_image_noise(seed, b, (4, h, w), 1 + pr.draws, *self.variation)
         return self.run_program(cond, uncond, pr.start(nz[0].to(self.device), init), pr, cfg_scale,
-                                noises=nz[1:] if pr.draws else None, inpaint=inpaint, controls=controls)
+                                noises=nz[1:] if pr.draws else None, inpaint=inpaint, controls=controls, tiling=tiling)
 
     @torch.no_grad()
     def txt2img_hires(self, tokens: torch.Tensor, neg_tokens: torch.Tensor, seed: int, steps: int = 20,
@@ -916,13 +924,14 @@ class SDEngine:
                       hr_steps: int = 0, denoising_strength: float = 0.7, sampler: str = "DDIM",
                       scheduler: Optional[str] = None, multipliers: Optional[torch.Tensor] = None,
                       neg_multipliers: Optional[torch.Tensor] = None, upscaler: str = "Latent",
-                      upscaler_tile: int = 192, upscaler_overlap: int = 8) -> torch.Tensor:
+                      upscaler_tile: int = 192, upscaler_overlap: int = 8, tiling: bool = False) -> torch.Tensor:
         """txt2img with sdwui's hires fix (StableDiffusionProcessingTxt2Img.sample / sample_hr_pass): first pass at
         (height, width), the `upscaler` to hr_scale x, a fresh per-image noise of the large shape from the same seeds,
         then the same sampler's img2img half from t_enc with `hr_steps` (0 = `steps`) steps, decode at the large size.
         `upscaler` (b200sd.upscale): a "Latent ..." mode resizes the latents (F.interpolate); any other name decodes the
         first pass, resizes the uint8 images as sdwui's images.resize_image does (ESRGAN tiles of `upscaler_tile` pixels
-        overlapping by `upscaler_overlap`) and VAE-encodes the result as img2img encodes init images.
+        overlapping by `upscaler_overlap`) and VAE-encodes the result as img2img encodes init images.  `tiling` holds for
+        both passes and the VAE decode / encode between them (the pixel upscalers are not part of the model).
         Returns uint8 [b, H*hr, W*hr, 3] on device."""
         from . import upscale
         kind, _ = upscale.kind(upscaler)
@@ -932,7 +941,7 @@ class SDEngine:
         if kind != "latent" and (int(height * hr_scale) % 8 or int(width * hr_scale) % 8):
             raise ValueError(f"hires upscaler {upscaler!r}: the target size must be a multiple of 8")
         cond, uncond = self._conds(tokens, neg_tokens, width, height, multipliers, neg_multipliers)
-        lat = self._sample_txt(cond, uncond, seed, b, h, w, steps, cfg_scale, sampler, scheduler)
+        lat = self._sample_txt(cond, uncond, seed, b, h, w, steps, cfg_scale, sampler, scheduler, tiling=tiling)
         if kind == "latent":
             with self._ctx():
                 if upscaler == "Latent":
@@ -942,33 +951,34 @@ class SDEngine:
                     up = upscale.resize_latents(lat, upscaler, h, w, h2, w2)
             init = up.reshape(b, h2, w2, 4).permute(0, 3, 1, 2)
         else:
-            images = self.decode(lat, h, w)
+            images = self.decode(lat, h, w, tiling)
             f = 2 ** (len(self.vae_cfg.ch_mult) - 1)   # 8 for the kl-f8 autoencoder: the target is then W*hr x H*hr
             with self._ctx():
                 images = upscale.resize_image(images, w2 * f, h2 * f, upscaler, upscaler_tile, upscaler_overlap)
-            init = self.encode(images.contiguous())
+            init = self.encode(images.contiguous(), tiling)
         if self.clip.xl:   # SDXL's vector conditioning carries the target size: the second pass gets its own (sdwui hr_c / hr_uc)
             cond, uncond = self._conds(tokens, neg_tokens, w2 * 8, h2 * 8, multipliers, neg_multipliers)
-        lat2 = self._sample_from(init, cond, uncond, seed, denoising_strength, hr_steps or steps, cfg_scale, sampler, scheduler)
-        return self.decode(lat2, h2, w2)
+        lat2 = self._sample_from(init, cond, uncond, seed, denoising_strength, hr_steps or steps, cfg_scale, sampler, scheduler,
+                                 tiling=tiling)
+        return self.decode(lat2, h2, w2, tiling)
 
     def _sample_txt(self, cond, uncond, seed: int, b: int, h: int, w: int, steps: int, cfg_scale: float, sampler: str,
-                    scheduler: Optional[str], controls=None) -> torch.Tensor:
+                    scheduler: Optional[str], controls=None, tiling: bool = False) -> torch.Tensor:
         pr = self.program(sampler, scheduler, steps)
         nz = per_image_noise(seed, b, (4, h, w), 1 + pr.draws, *self.variation)
         return self.run_program(cond, uncond, pr.start(nz[0]), pr, cfg_scale, noises=nz[1:] if pr.draws else None,
-                                controls=controls)
+                                controls=controls, tiling=tiling)
 
     @torch.no_grad()
     def txt2img(self, tokens: torch.Tensor, neg_tokens: torch.Tensor, seed: int, steps: int = 20, cfg_scale: float = 7.0,
                 height: int = 512, width: int = 512, sampler: str = "DDIM", scheduler: Optional[str] = None,
                 multipliers: Optional[torch.Tensor] = None, neg_multipliers: Optional[torch.Tensor] = None,
-                controls=None) -> torch.Tensor:
+                controls=None, tiling: bool = False) -> torch.Tensor:
         """Whole request for this engine's share: returns uint8 [b, H, W, 3] on device.  tokens [b, 77 * k] and
         neg_tokens [b, 77 * k'] with their optional emphasis multipliers of the same shapes (factory.tokenize_prompts).
-        `controls`: ControlNet units as for img2img (None: none)."""
+        `controls`: ControlNet units as for img2img (None: none); `tiling` as for img2img."""
         b = tokens.shape[0]
         h, w = height // 8, width // 8
         cond, uncond = self._conds(tokens, neg_tokens, width, height, multipliers, neg_multipliers)
-        lat = self._sample_txt(cond, uncond, seed, b, h, w, steps, cfg_scale, sampler, scheduler, controls)
-        return self.decode(lat, h, w)
+        lat = self._sample_txt(cond, uncond, seed, b, h, w, steps, cfg_scale, sampler, scheduler, controls, tiling)
+        return self.decode(lat, h, w, tiling)

@@ -208,6 +208,20 @@ def upsample2x(x: torch.Tensor, out: torch.Tensor):
     return out
 
 
+def pad_circular(x: torch.Tensor, out: torch.Tensor, p: int):
+    """x [NB, H, W, C] NHWC (pixel pitch x.stride(2)) -> out [NB, H+2p, W+2p, C]: x inside, the halo copied from the
+    opposite edges (F.pad(mode="circular")).  p > H or p > W is refused."""
+    nb, h, w, c = x.shape
+    for t in (x, out):
+        assert t.stride(3) == 1 and t.stride(1) == t.shape[2] * t.stride(2) and t.stride(0) == t.shape[1] * t.stride(1)
+    assert out.shape == (nb, h + 2 * p, w + 2 * p, c) and out.dtype == x.dtype, (tuple(x.shape), tuple(out.shape), p)
+    rc = _lib.lib().b200sd_pad_circular(_p(x), ctypes.c_longlong(x.stride(2)), _p(out), ctypes.c_longlong(out.stride(2)),
+                                        nb, h, w, c, p, _dt(x), _stream())
+    check(rc, f"b200sd_pad_circular NB={nb} H={h} W={w} C={c} p={p}")
+    _count()
+    return out
+
+
 def softmax_rows_(s: torch.Tensor, scale: float):
     rows, cols, lds = _rows2d(s)
     rc = _lib.lib().b200sd_softmax_rows(_p(s), ctypes.c_longlong(lds), rows, cols, ctypes.c_float(scale), _dt(s),

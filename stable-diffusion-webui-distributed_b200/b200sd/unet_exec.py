@@ -200,6 +200,20 @@ def _pad_to(c: int, m: int) -> int:
     return -(-c // m) * m
 
 
+def emit_conv3(prog, x: torch.Tensor, h: int, wd: int, *a, **k):
+    """emit a 3x3 conv with padding 1 on x [n, h*wd, C] into `prog` (a UNet or VAE program: its `_emit`, `pool` and
+    `circular`).  Zero padding is the conv kernel's own; with `prog.circular` (sdwui's tiling) it is circular: x is
+    copied into pool scratch one pixel larger on each side with the halo wrapped around (ops.pad_circular), and the conv
+    reads that with no padding.  Stride 2 then gives the same output size as zero padding 1."""
+    if not prog.circular:
+        prog._emit(ops.conv2d, x.unflatten(1, (h, wd)), *a, ksize=3, **k)
+        return
+    xp = prog.pool.get(x.shape[0], (h + 2) * (wd + 2), x.shape[-1])
+    prog._emit(ops.pad_circular, x.unflatten(1, (h, wd)), xp.unflatten(1, (h + 2, wd + 2)), 1)
+    prog._emit(ops.conv2d, xp.unflatten(1, (h + 2, wd + 2)), *a, ksize=3, pad=0, **k)
+    prog.pool.put(xp)
+
+
 class ControlNetWeights(UNetWeights):
     """An ldm ControlNet (keys `control_model.*`, factory.controlnet) packed for a UNet of config `cfg`: its time
     embedding, input blocks and middle block go through UNetWeights' packers under the same names (`input_blocks.1.0.
@@ -229,8 +243,10 @@ class ControlNetWeights(UNetWeights):
 class UNetProgram:
     """One UNet evaluation for a fixed (N, H, W): `run()` launches ~700 kernels, no allocation, no sync."""
 
-    def __init__(self, w: UNetWeights, n: int, h: int, wd: int, ctx_len: int = 77):
+    def __init__(self, w: UNetWeights, n: int, h: int, wd: int, ctx_len: int = 77, tiling: bool = False):
+        """tiling: every 3x3 conv of the UNet pads circularly (sdwui's tiling option); ControlNet segments never do"""
         self.w, self.cfg = w, w.cfg
+        self.tiling = self.circular = tiling
         self.n, self.h, self.wd = n, h, wd
         self.dev, self.dt = w.device, w.dtype
         self.pool = Pool(self.dev, self.dt)
@@ -321,11 +337,14 @@ class UNetProgram:
         saved = (self.w, self.cur_bias, self.ctx_kv, self._xattn, self.ops, self.op_flops, self.gn_elems, self.ln_elems)
         self.w, self.cur_bias, self.ctx_kv, self._xattn, self.ops, self.op_flops = \
             seg.w, seg.cur_bias, seg.ctx_kv, seg.xattn, seg.ops, seg.op_flops
+        # sd-webui-controlnet's model is not part of the sd model that sdwui's tiling makes circular: zero padding
+        self.circular = False
         try:
             yield
         finally:
             (self.w, self.cur_bias, self.ctx_kv, self._xattn, self.ops, self.op_flops, self.gn_elems,
              self.ln_elems) = saved
+            self.circular = self.tiling
 
     def _run_layers(self, prefix, layers, x, h, wd, final_dest, conv_in_residual=None):
         """x: input view; the LAST layer writes into final_dest (a view with the right channel count).  conv_in reads the
@@ -339,8 +358,8 @@ class UNetProgram:
             tmp = None
             if kind == "conv_in":
                 dest = final_dest
-                self._emit(ops.conv2d, self.xin.unflatten(1, (h, wd)), t[key + ".w"], dest, ksize=3, bias=t[key + ".b"],
-                           residual=conv_in_residual, algo_flops=2.0 * n * h * wd * 9 * cfg.in_channels * layer[2])
+                emit_conv3(self, self.xin, h, wd, t[key + ".w"], dest, bias=t[key + ".b"], residual=conv_in_residual,
+                           algo_flops=2.0 * n * h * wd * 9 * cfg.in_channels * layer[2])
             elif kind == "res":
                 dest = final_dest if last else self.pool.get(n, h * wd, layer[2])
                 tmp = None if last else dest
@@ -351,14 +370,14 @@ class UNetProgram:
                 self._attn(key, x, layer[1], layer[2], h, wd, dest)
             elif kind == "down":
                 dest = final_dest
-                self._emit(ops.conv2d, x.unflatten(1, (h, wd)), t[key + ".w"], dest, ksize=3, stride=2, bias=t[key + ".b"])
+                emit_conv3(self, x, h, wd, t[key + ".w"], dest, stride=2, bias=t[key + ".b"])
                 h, wd = (h + 1) // 2, (wd + 1) // 2
             elif kind == "up":
                 up = self.pool.get(n, 4 * h * wd, layer[1])
                 self._emit(ops.upsample2x, x.unflatten(1, (h, wd)), up.unflatten(1, (2 * h, 2 * wd)))
                 h, wd = 2 * h, 2 * wd
                 dest = final_dest
-                self._emit(ops.conv2d, up.unflatten(1, (h, wd)), t[key + ".w"], dest, ksize=3, bias=t[key + ".b"])
+                emit_conv3(self, up, h, wd, t[key + ".w"], dest, bias=t[key + ".b"])
                 self.pool.put(up)
             if prev_tmp is not None:  # the previous layer's scratch output has now been consumed
                 self.pool.put(prev_tmp)
@@ -389,11 +408,10 @@ class UNetProgram:
         b = self.pool.get(n, hw, cout)
         if self.per_sample:   # a bias row per image: rows [i * hw, (i + 1) * hw) of the GEMM take row i
             bsl = self.cur_bias[n * off: n * (off + cout)]
-            self._emit(ops.conv2d, a.unflatten(1, (h, wd)), t[key + ".conv1.w"], b.reshape(n * hw, cout), ksize=3, bias=bsl,
-                       bias_group_rows=hw)
+            emit_conv3(self, a, h, wd, t[key + ".conv1.w"], b.reshape(n * hw, cout), bias=bsl, bias_group_rows=hw)
         else:
             bsl = self.cur_bias[off: off + cout]
-            self._emit(ops.conv2d, a.unflatten(1, (h, wd)), t[key + ".conv1.w"], b.reshape(n * hw, cout), ksize=3, bias=bsl)
+            emit_conv3(self, a, h, wd, t[key + ".conv1.w"], b.reshape(n * hw, cout), bias=bsl)
         self.pool.put(a)
         c = self.pool.get(n, hw, cout)
         self._gn(b, c, key + ".gn2", 1e-5, True)
@@ -404,8 +422,7 @@ class UNetProgram:
             skip = s
         else:
             s, skip = None, x
-        self._emit(ops.conv2d, c.unflatten(1, (h, wd)), t[key + ".conv2.w"], dest, ksize=3, bias=t[key + ".conv2.b"],
-                   residual=skip)
+        emit_conv3(self, c, h, wd, t[key + ".conv2.w"], dest, bias=t[key + ".conv2.b"], residual=skip)
         self.pool.put(c)
         if s is not None:
             self.pool.put(s)
@@ -515,8 +532,8 @@ class UNetProgram:
         # ---- out: GN + SiLU + conv3x3 -> eps (4 channels padded to 32)
         a = self.pool.get(n, self.h * self.wd, cfg.model_channels)
         self._gn(final, a, "out.gn", 1e-5, True)
-        self._emit(ops.conv2d, a.unflatten(1, (self.h, self.wd)), t["out.conv.w"], self.eps.reshape(-1, 32), ksize=3,
-                   bias=t["out.conv.b"], algo_flops=2.0 * n * self.h * self.wd * 9 * cfg.model_channels * cfg.out_channels)
+        emit_conv3(self, a, self.h, self.wd, t["out.conv.w"], self.eps.reshape(-1, 32), bias=t["out.conv.b"],
+                   algo_flops=2.0 * n * self.h * self.wd * 9 * cfg.model_channels * cfg.out_channels)
         self.pool.put(a)
 
     # ---------------------------------------------------------------- execution

@@ -15,7 +15,7 @@ import torch
 
 from . import ops
 from .config import VAE_PREFIX, VAEConfig
-from .unet_exec import Pool
+from .unet_exec import Pool, emit_conv3
 from .weights import pack_conv
 
 
@@ -119,8 +119,10 @@ class VAEEncoderWeights:
 class _VAEProgram:
     """Shared layer emitters: every op is recorded once, run() replays them (allocation- and sync-free)."""
 
-    def __init__(self, weights, b: int):
+    def __init__(self, weights, b: int, tiling: bool = False):
+        """tiling: every 3x3 conv with padding 1 pads circularly (sdwui's tiling option)"""
         self.w, self.b = weights, b
+        self.circular = tiling
         self.dev, self.dt = weights.device, weights.dtype
         self.pool = Pool(self.dev, self.dt)
         self.ops: List = []
@@ -148,7 +150,7 @@ class _VAEProgram:
         a = self.pool.get(b, hw, cin)
         self._gn(x, a, name + ".gn1", True)
         c1 = self.pool.get(b, hw, cout)
-        self._emit(ops.conv2d, a.unflatten(1, (h, wd)), t[name + ".conv1.w"], c1, ksize=3, bias=t[name + ".conv1.b"])
+        emit_conv3(self, a, h, wd, t[name + ".conv1.w"], c1, bias=t[name + ".conv1.b"])
         self.pool.put(a)
         a2 = self.pool.get(b, hw, cout)
         self._gn(c1, a2, name + ".gn2", True)
@@ -159,8 +161,7 @@ class _VAEProgram:
         else:
             s = x
         out = self.pool.get(b, hw, cout)
-        self._emit(ops.conv2d, a2.unflatten(1, (h, wd)), t[name + ".conv2.w"], out, ksize=3, bias=t[name + ".conv2.b"],
-                   residual=s)
+        emit_conv3(self, a2, h, wd, t[name + ".conv2.w"], out, bias=t[name + ".conv2.b"], residual=s)
         self.pool.put(a2)
         if s is not x:
             self.pool.put(s)
@@ -203,8 +204,8 @@ class _VAEProgram:
 class VAEDecoderProgram(_VAEProgram):
     """Decode `b` latents of size h x w -> uint8 [b, 8h*.., 3]."""
 
-    def __init__(self, w: VAEDecoderWeights, b: int, h: int, wd: int):
-        super().__init__(w, b)
+    def __init__(self, w: VAEDecoderWeights, b: int, h: int, wd: int, tiling: bool = False):
+        super().__init__(w, b, tiling)
         self.h, self.wd = h, wd
         self.zin = torch.zeros((2 * b, h * wd, 64), device=self.dev, dtype=self.dt)  # pack_unet_input writes both halves
         self._build()
@@ -216,7 +217,7 @@ class VAEDecoderProgram(_VAEProgram):
         z = self.pool.get(b, h * wd, 64)
         self._emit(ops.linear, self.zin[:b], t["post_quant.w"], z, bias=t["post_quant.b"])
         x = self.pool.get(b, h * wd, c)
-        self._emit(ops.conv2d, z.unflatten(1, (h, wd)), t["conv_in.w"], x, ksize=3, bias=t["conv_in.b"])
+        emit_conv3(self, z, h, wd, t["conv_in.w"], x, bias=t["conv_in.b"])
         self.pool.put(z)
         x = self._mid(x, c, h, wd)
         for lvl, blocks in self.w.levels:
@@ -231,14 +232,13 @@ class VAEDecoderProgram(_VAEProgram):
                 self.pool.put(x)
                 h, wd = 2 * h, 2 * wd
                 x = self.pool.get(b, h * wd, c)
-                self._emit(ops.conv2d, up.unflatten(1, (h, wd)), t[f"up{lvl}.upsample.w"], x, ksize=3,
-                           bias=t[f"up{lvl}.upsample.b"])
+                emit_conv3(self, up, h, wd, t[f"up{lvl}.upsample.w"], x, bias=t[f"up{lvl}.upsample.b"])
                 self.pool.put(up)
         a = self.pool.get(b, h * wd, c)
         self._gn(x, a, "norm_out", True)
         self.pool.put(x)
         self.img = torch.empty((b, h * wd, 32), device=self.dev, dtype=self.dt)   # RGB in channels 0..2, in [-1, 1]
-        self._emit(ops.conv2d, a.unflatten(1, (h, wd)), t["conv_out.w"], self.img, ksize=3, bias=t["conv_out.b"])
+        emit_conv3(self, a, h, wd, t["conv_out.w"], self.img, bias=t["conv_out.b"])
         self.pool.put(a)
         self.out_h, self.out_w = h, wd
         self.u8 = torch.empty((b, h * wd, 3), device=self.dev, dtype=torch.uint8)
@@ -256,8 +256,8 @@ class VAEDecoderProgram(_VAEProgram):
 class VAEEncoderProgram(_VAEProgram):
     """Encode `b` RGB images of size H x W (uint8) -> scaled latents fp32 [b, (H/f)*(W/f), 4] (posterior mean)."""
 
-    def __init__(self, w: VAEEncoderWeights, b: int, height: int, width: int):
-        super().__init__(w, b)
+    def __init__(self, w: VAEEncoderWeights, b: int, height: int, width: int, tiling: bool = False):
+        super().__init__(w, b, tiling)
         self.height, self.width = height, width
         self.img_u8 = torch.zeros((b, height * width, 3), device=self.dev, dtype=torch.uint8)
         self.xin = torch.zeros((b, height * width, 64), device=self.dev, dtype=self.dt)  # RGB in channels 0..2
@@ -269,7 +269,7 @@ class VAEEncoderProgram(_VAEProgram):
         self._emit(ops.image_to_nhwc, self.img_u8, self.xin)
         c = self.w.cfg.ch
         x = self.pool.get(b, h * wd, c)
-        self._emit(ops.conv2d, self.xin.unflatten(1, (h, wd)), t["conv_in.w"], x, ksize=3, bias=t["conv_in.b"])
+        emit_conv3(self, self.xin, h, wd, t["conv_in.w"], x, bias=t["conv_in.b"])
         nlev = len(self.w.levels)
         for lvl, blocks in self.w.levels:
             for i, (cin, cout) in enumerate(blocks):
@@ -280,6 +280,7 @@ class VAEEncoderProgram(_VAEProgram):
             if lvl != nlev - 1:
                 ho, wo = h // 2, wd // 2
                 y = self.pool.get(b, ho * wo, c)
+                # F.pad((0, 1, 0, 1)) with zeros, then a conv with padding 0: tiling leaves it as it is
                 self._emit(ops.conv2d, x.unflatten(1, (h, wd)), t[f"down{lvl}.downsample.w"], y, ksize=3, stride=2, pad=0,
                            pad_end=1, bias=t[f"down{lvl}.downsample.b"])
                 self.pool.put(x)
@@ -289,7 +290,7 @@ class VAEEncoderProgram(_VAEProgram):
         self._gn(x, a, "norm_out", True)
         self.pool.put(x)
         m = self.pool.get(b, h * wd, 64)
-        self._emit(ops.conv2d, a.unflatten(1, (h, wd)), t["conv_out.w"], m, ksize=3, bias=t["conv_out.b"])
+        emit_conv3(self, a, h, wd, t["conv_out.w"], m, bias=t["conv_out.b"])
         self.pool.put(a)
         moments = self.pool.get(b, h * wd, 64)
         self._emit(ops.linear, m, t["quant.w"], moments, bias=t["quant.b"])

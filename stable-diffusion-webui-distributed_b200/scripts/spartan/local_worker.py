@@ -228,6 +228,9 @@ class LocalGPUWorker(Worker):
         weights = {"neg_multipliers": neg_mult} if weighted(neg_mult) else {}
         if controls:   # a payload without ControlNet units reaches the engine with exactly the arguments it always had
             weights["controls"] = controls
+        tiling = self._tiling(payload)
+        if tiling:     # likewise an untiled payload
+            weights["tiling"] = True
         chunks = []
         for it in range(n_iter):
             # variation seeds: image k of iteration `it` blends noise(seed + k) with noise(subseed + k)
@@ -287,7 +290,7 @@ class LocalGPUWorker(Worker):
         seeds = [seed + (i if strength == 0 else 0) for i in range(n)]
         subseeds = [subseed + i for i in range(n)]
         infotexts = [f"{prompt}\nNegative prompt: {negative}\nSteps: {steps}, Sampler: {sampler}, CFG scale: {cfg_scale}, "
-                     f"Seed: {s}, Size: {width}x{height}" for s in seeds]
+                     f"Seed: {s}, Size: {width}x{height}" + (", Tiling: True" if tiling else "") for s in seeds]
         info = {"all_seeds": seeds, "all_subseeds": subseeds, "all_prompts": [prompt] * n,
                 "all_negative_prompts": [negative] * n, "infotexts": infotexts, "seed": seeds[0], "subseed": subseeds[0],
                 "prompt": prompt, "negative_prompt": negative}
@@ -322,6 +325,19 @@ class LocalGPUWorker(Worker):
             if opts.get("ESRGAN_tile_overlap") is not None:
                 out["upscaler_overlap"] = int(opts["ESRGAN_tile_overlap"])
         return out
+
+    @staticmethod
+    def _tiling(payload: dict) -> bool:
+        """sdwui's tiling setting of the request: the payload's `tiling` unless it is None, then the request's
+        override_settings, then the options of the sdwui this runs in (sdwui >= 1.6 leaves p.tiling None until
+        process_images_inner reads opts.tiling; a host without that option gives False)"""
+        value = payload.get("tiling")
+        if value is None:
+            value = (payload.get("override_settings") or {}).get("tiling")
+        if value is None:
+            import modules.shared
+            value = getattr(getattr(modules.shared, "opts", None), "tiling", False)
+        return bool(value)
 
     def _controls(self, eng, payload: dict, width: int, height: int):
         """the payload's enabled ControlNet units as SDEngine `controls` (None: no unit); refusals raise ValueError"""
