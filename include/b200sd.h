@@ -203,6 +203,18 @@ int b200sd_image_to_nhwc(const unsigned char* img, void* out, long long pitch, i
  * ControlNet input_hint_block input, sd-webui-controlnet's HWC3(image) / 255).  Not 2x/255 - 1: the hint block's zero
  * padding at the image borders must stand for black. */
 int b200sd_hint_to_nhwc(const unsigned char* img, void* out, long long pitch, int B, int HW, int dtype, void* stream);
+/* inpainting-model conditioning image: uint8 [B,HW,3] RGB and mask uint8 [HW] (NULL: all ones) -> [B,HW,pitch] with
+ * channel c < 3 = (2*x/255 - 1) * (1 - weight * [mask >= 128]) (channels >= 3 untouched).  sdwui
+ * inpainting_image_conditioning: torch.lerp(s, s * (1 - M), inpainting_mask_weight), M = round(mask / 255).  Where the mask
+ * is 0 the output is bitwise b200sd_image_to_nhwc's. */
+int b200sd_masked_image_to_nhwc(const unsigned char* img, const unsigned char* mask, float weight, void* out,
+                                long long pitch, int B, int HW, int dtype, void* stream);
+/* inpainting-model UNet input: z fp32 [B,h*w,4] (VAE latents of the conditioning image) and the pixel mask uint8
+ * [f*h, f*w] (NULL: all ones) -> channel 4 = [mask[f*i, f*j] >= 128] (nearest F.interpolate to the latent size) and
+ * channels 5..8 = z of rows b and B+b of xin [2B,h*w,pitch] ([cond | uncond]).  No other channel is touched.
+ * pitch >= 9 and pitch % 4 == 0, z 16-byte and xin 8-byte aligned. */
+int b200sd_pack_image_cond(const float* z, const unsigned char* mask, void* xin, long long pitch, int B, int h, int w,
+                           int f, int dtype, void* stream);
 /* VAE encoder moments [B,HW,pitch] (first 4 channels = posterior mean) -> scaled latents fp32 [B,HW,4] = mean * scale
  * (AutoencoderKL.encode(...).mean * scale_factor) */
 int b200sd_unpack_latent(const void* moments, long long pitch, float* x, int B, int HW, float scale, int dtype,

@@ -15,7 +15,7 @@ import torch
 from . import ops
 from . import samplers as S
 from .clip_text import CAPTURE_LOCK as _CAPTURE_LOCK, Cond, Conditioner
-from .config import CLIPConfig, UNetConfig, VAEConfig
+from .config import UNET_PREFIX, CLIPConfig, UNetConfig, VAEConfig
 from .unet_exec import MAX_CONTROLS, ControlNetWeights, TimeEmbedding, UNetProgram, UNetWeights
 from .vae_exec import VAEDecoderProgram, VAEDecoderWeights, VAEEncoderProgram, VAEEncoderWeights
 
@@ -25,6 +25,8 @@ MAX_GRAPHS = 48      # step graphs kept per plan (one per sampler stage structur
 CHUNK = 77           # tokens per prompt chunk (sdwui: [BOS] + 75 + [EOS]); contexts are 77 * k tokens long
 NOISE_SAMPLERS = ("Euler a", "stage")   # graph-name prefixes of the step graphs that may read Plan.noise
 PREDICTIONS = ("eps", "v")   # what the UNet predicts: the noise (SD1.x, SDXL, SD 2.x-base) or v (SD 2.x 768-v)
+# UNet input channels served: the latents (4), or latents + mask + masked-image latents (9, inpainting checkpoints)
+IN_CHANNELS = (4, 9)
 # _CAPTURE_LOCK (imported): CUDA graph captures are serialised across the per-device worker threads
 
 
@@ -413,10 +415,17 @@ class SDEngine:
         """prediction: "eps" (the UNet predicts the noise) or "v" (v-parameterisation, SD 2.x 768-v and v finetunes)"""
         if prediction not in PREDICTIONS:
             raise ValueError(f"prediction {prediction!r} is not one of {PREDICTIONS}")
+        if unet_cfg.in_channels not in IN_CHANNELS:
+            raise ValueError(f"a UNet with {unet_cfg.in_channels} input channels is not served: only 4-channel models and "
+                             f"9-channel inpainting models are (not instruct-pix2pix's 8 or depth2img's 5)")
         self.prediction = prediction
         self.device = torch.device(device)
         if self.device.type != "cuda" and self._require_cuda:
             raise RuntimeError("SDEngine needs a CUDA device: the hot path is sm_90a kernels only (no CPU fallback)")
+        w_in = sd[UNET_PREFIX + "input_blocks.0.0.weight"].shape[1]
+        if w_in != unet_cfg.in_channels:
+            raise ValueError(f"the UNet config takes {unet_cfg.in_channels} input channels but the checkpoint's conv_in "
+                             f"takes {w_in}")
         self.dtype = dtype
         self.unet_cfg, self.vae_cfg, self.clip_cfg = unet_cfg, vae_cfg, clip_cfg
         self.use_graphs = use_graphs
@@ -436,6 +445,11 @@ class SDEngine:
         self._cap_stream = None
         self.last_unet_evals = 0
         self.graph_replayed_launches = 0   # b200sd kernels launched through graph replays (bench.py gpu_launches)
+
+    @property
+    def inpainting(self) -> bool:
+        """a 9-channel inpainting UNet: every sampling run packs its image conditioning (mask, masked-image latents)"""
+        return self.unet_cfg.in_channels == 9
 
     def _capture_stream(self):
         """torch.cuda.graph's default capture stream is ONE process-wide stream, created on whichever device captured
@@ -636,15 +650,20 @@ class SDEngine:
     @torch.no_grad()
     def run_program(self, cond: torch.Tensor, uncond: torch.Tensor, x_start: torch.Tensor, pr: "Program", cfg_scale: float,
                     noises: Optional[torch.Tensor] = None, inpaint=None, controls=None,
-                    tiling: bool = False) -> torch.Tensor:
+                    tiling: bool = False, image_cond=None) -> torch.Tensor:
         """cond/uncond [b, 77 * k, ctx] on device (cond and uncond may have different k); x_start [b, 4, h, w] fp32 (host or device) = Program.start(...): the start
         latents in the sampler's own space; noises [pr.draws, b, 4, h, w]: the per-image N(0,1) draws after the first;
         inpaint = (clean init latents [b, 4, h, w], latent mask [h * w]).  controls: ControlNet units, see _set_controls
-        (None: no ControlNet).  tiling: the UNet's convs pad circularly (its own plan).  Returns the final latents fp32
-        [b, h*w, 4] (NHWC, a view of plan state)."""
+        (None: no ControlNet).  tiling: the UNet's convs pad circularly (its own plan).  image_cond = (masked-image
+        latents fp32 [b, 4, h, w], pixel mask uint8 [f*h, f*w] or None for all ones): an inpainting model's extra UNet
+        input channels, packed once before sampling (required for a 9-channel UNet, refused for a 4-channel one).  Returns
+        the final latents fp32 [b, h*w, 4] (NHWC, a view of plan state)."""
         b, _, h, w = x_start.shape
         if pr.draws and (noises is None or noises.shape[0] < pr.draws):
             raise ValueError(f"{pr.sampler} needs {pr.draws} per-image noise draws")
+        if (image_cond is not None) != self.inpainting:
+            raise ValueError("an inpainting model samples with its image conditioning" if self.inpainting else
+                             "image conditioning is for 9-channel inpainting models only")
         if inpaint is not None and pr.fused not in (None, "ddim"):
             # the fused Euler / Euler a / DPM++ 2M kernels do not carry the mask: same sampler, generic stages
             raise ValueError("masked sampling of a fused sampler must be requested through a generic program")
@@ -662,6 +681,10 @@ class SDEngine:
             if masked:   # (clean init latents [b, 4, h, w], latent mask [h * w])
                 plan.init.copy_(inpaint[0].to(self.device, torch.float32).permute(0, 2, 3, 1).reshape(b, h * w, 4))
                 plan.latmask.copy_(inpaint[1].to(self.device, torch.float32).reshape(-1))
+            if image_cond is not None:   # channels 4..8 of [cond | uncond]; the step kernels write channels 0..3 only
+                z, m = image_cond
+                ops.pack_image_cond(z.to(self.device, torch.float32).permute(0, 2, 3, 1).reshape(b, h * w, 4).contiguous(),
+                                    None if m is None else m.to(self.device, torch.uint8).contiguous(), plan.unet.xin, h, w)
             plan.x.copy_(x_start.to(self.device, torch.float32).permute(0, 2, 3, 1).reshape(b, h * w, 4))
             plan.step.zero_()
             ops.pack_unet_input(plan.x, plan.unet.xin, pr.in0)
@@ -853,15 +876,33 @@ class SDEngine:
     def encode(self, images_u8: torch.Tensor, tiling: bool = False) -> torch.Tensor:
         """images uint8 [b, H, W, 3] (host or device) -> scaled latents fp32 [b, 4, H/f, W/f] (posterior mean), in
         chunks of `vae_chunk` images.  tiling: circular convs (an encoder program of its own)."""
+        return self._encode(images_u8, tiling)
+
+    @torch.no_grad()
+    def encode_conditioning(self, images_u8: torch.Tensor, mask_u8: Optional[torch.Tensor] = None, weight: float = 1.0,
+                            tiling: bool = False) -> torch.Tensor:
+        """the masked-image half of an inpainting model's conditioning (sdwui inpainting_image_conditioning): uint8
+        images [b, H, W, 3] and the pixel mask uint8 [H, W] (None: all ones) -> scaled latents fp32 [b, 4, H/f, W/f] of
+        s * (1 - weight * [mask >= 128]), s = 2x/255 - 1, encoded as `encode` encodes init images"""
+        return self._encode(images_u8, tiling, (mask_u8, weight))
+
+    def _encode(self, images_u8: torch.Tensor, tiling: bool, condition=None) -> torch.Tensor:
+        """encode / encode_conditioning; condition = (mask, weight) runs the masked encoder program of the size"""
         b, hh, ww, _ = images_u8.shape
         with self._ctx():
             c = min(self.vae_chunk, b)
             key = (c, hh, ww, "tiling") if tiling else (c, hh, ww)
+            if condition is not None:
+                key = key + ("masked",)
             if key not in self.encoders:
                 while len(self.encoders) >= MAX_PLANS:
                     self.encoders.pop(next(iter(self.encoders)))
-                self.encoders[key] = VAEEncoderProgram(self.vae_enc_w, c, hh, ww, tiling=tiling)
+                self.encoders[key] = VAEEncoderProgram(self.vae_enc_w, c, hh, ww, tiling=tiling,
+                                                       masked=condition is not None)
             enc = self.encoders[key]
+            if condition is not None:
+                mask, weight = condition
+                enc.set_condition(None if mask is None else mask.to(self.device, torch.uint8), weight)
             imgs = images_u8.to(self.device).reshape(b, hh * ww, 3)
             out = torch.empty((b, enc.lat_h * enc.lat_w, 4), device=self.device, dtype=torch.float32)
             for i in range(0, b, c):
@@ -879,7 +920,8 @@ class SDEngine:
                 denoising_strength: float = 0.75, steps: int = 20, cfg_scale: float = 7.0, sampler: str = "DDIM",
                 scheduler: Optional[str] = None, latmask: Optional[torch.Tensor] = None,
                 inpainting_fill: int = 1, multipliers: Optional[torch.Tensor] = None,
-                neg_multipliers: Optional[torch.Tensor] = None, controls=None, tiling: bool = False) -> torch.Tensor:
+                neg_multipliers: Optional[torch.Tensor] = None, controls=None, tiling: bool = False,
+                image_mask: Optional[torch.Tensor] = None, inpainting_mask_weight: float = 1.0) -> torch.Tensor:
         """img2img: VAE-encode the init images (posterior mean), noise them to t_enc, run the remaining part of the
         sampler's schedule, decode.  init_u8 uint8 [b, H, W, 3].  Returns uint8 [b, H, W, 3] on device.
         `latmask` fp32 [h * w] (b200sd.inpaint.prepare_mask): inpainting — the region with latmask 0 is held to the init
@@ -892,23 +934,41 @@ class SDEngine:
         `controls`: ControlNet units [(ControlNetWeights, control map uint8 [H, W, 3], weight, guidance_start,
         guidance_end)], at most 3 (None: none).
         `tiling`: sdwui's tiling option — every 3x3 conv of the UNet and the VAE pads circularly (ControlNet's do
-        not)."""
+        not).
+        Inpainting models (9 input channels) are conditioned on the mask and the VAE latents of
+        init * (1 - inpainting_mask_weight * mask) (sdwui img2img_image_conditioning): `image_mask` uint8 [H, W] is the
+        processed pixel mask (inpaint.InpaintMask.fill_mask), required with `latmask`; without a mask it is all ones.
+        Other models ignore both arguments."""
         b = tokens.shape[0]
         cond, uncond = self._conds(tokens, neg_tokens, init_u8.shape[2], init_u8.shape[1], multipliers, neg_multipliers)
         init = self.encode(init_u8, tiling)
         _, _, h, w = init.shape
+        image_cond = None
+        if self.inpainting:
+            if latmask is not None and image_mask is None:
+                raise ValueError("masked img2img on an inpainting model needs the pixel mask (image_mask)")
+            image_cond = (self.encode_conditioning(init_u8, image_mask, inpainting_mask_weight, tiling), image_mask)
         if latmask is not None and inpainting_fill in (2, 3):
             nm = latmask.to(self.device, torch.float32).reshape(1, 1, h, w)
             init = init * (1.0 - nm)
             if inpainting_fill == 2:   # create_random_tensors(shape, seeds): the same first draw the sampler starts from
                 init = init + per_image_noise(seed, b, (4, h, w), 1, *self.variation)[0].to(self.device) * nm
         lat = self._sample_from(init, cond, uncond, seed, denoising_strength, steps, cfg_scale, sampler, scheduler,
-                                inpaint=None if latmask is None else (init, latmask), controls=controls, tiling=tiling)
+                                inpaint=None if latmask is None else (init, latmask), controls=controls, tiling=tiling,
+                                image_cond=image_cond)
         return self.decode(lat, h, w, tiling)
+
+    def _txt2img_cond(self, b: int, h: int, w: int, tiling: bool):
+        """sdwui txt2img_image_conditioning of an inpainting model at latent size h x w: an all-ones mask over a gray image
+        (0 in [-1, 1]).  Weight 1 under the all-ones mask zeroes every pixel, so one image of any content (255: +0) is
+        encoded and shared by the b images."""
+        f = 2 ** (len(self.vae_cfg.ch_mult) - 1)
+        gray = torch.full((1, f * h, f * w, 3), 255, device=self.device, dtype=torch.uint8)
+        return self.encode_conditioning(gray, None, 1.0, tiling).expand(b, -1, -1, -1), None
 
     def _sample_from(self, init: torch.Tensor, cond, uncond, seed: int, denoising_strength: float, steps: int,
                      cfg_scale: float, sampler: str, scheduler: Optional[str], inpaint=None, controls=None,
-                     tiling: bool = False) -> torch.Tensor:
+                     tiling: bool = False, image_cond=None) -> torch.Tensor:
         """the img2img half of a sampler (also the second pass of the hires fix): `init` [b, 4, h, w] latents on the device,
         fresh per-image noise from `seed`, start at the noise level of t_enc.
         DDIM / PLMS: sdwui sd_samplers_timesteps.sample_img2img; k-diffusion samplers: KDiffusionSampler.sample_img2img."""
@@ -916,7 +976,8 @@ class SDEngine:
         pr = self.program(sampler, scheduler, steps, denoise=denoising_strength, masked=inpaint is not None)
         nz = per_image_noise(seed, b, (4, h, w), 1 + pr.draws, *self.variation)
         return self.run_program(cond, uncond, pr.start(nz[0].to(self.device), init), pr, cfg_scale,
-                                noises=nz[1:] if pr.draws else None, inpaint=inpaint, controls=controls, tiling=tiling)
+                                noises=nz[1:] if pr.draws else None, inpaint=inpaint, controls=controls, tiling=tiling,
+                                image_cond=image_cond)
 
     @torch.no_grad()
     def txt2img_hires(self, tokens: torch.Tensor, neg_tokens: torch.Tensor, seed: int, steps: int = 20,
@@ -924,7 +985,8 @@ class SDEngine:
                       hr_steps: int = 0, denoising_strength: float = 0.7, sampler: str = "DDIM",
                       scheduler: Optional[str] = None, multipliers: Optional[torch.Tensor] = None,
                       neg_multipliers: Optional[torch.Tensor] = None, upscaler: str = "Latent",
-                      upscaler_tile: int = 192, upscaler_overlap: int = 8, tiling: bool = False) -> torch.Tensor:
+                      upscaler_tile: int = 192, upscaler_overlap: int = 8, tiling: bool = False,
+                      inpainting_mask_weight: float = 1.0) -> torch.Tensor:
         """txt2img with sdwui's hires fix (StableDiffusionProcessingTxt2Img.sample / sample_hr_pass): first pass at
         (height, width), the `upscaler` to hr_scale x, a fresh per-image noise of the large shape from the same seeds,
         then the same sampler's img2img half from t_enc with `hr_steps` (0 = `steps`) steps, decode at the large size.
@@ -932,16 +994,24 @@ class SDEngine:
         first pass, resizes the uint8 images as sdwui's images.resize_image does (ESRGAN tiles of `upscaler_tile` pixels
         overlapping by `upscaler_overlap`) and VAE-encodes the result as img2img encodes init images.  `tiling` holds for
         both passes and the VAE decode / encode between them (the pixel upscalers are not part of the model).
+        Inpainting models: the first pass and a "Latent" second pass get txt2img's conditioning, a pixel upscaler's second
+        pass the upscaled images' under an all-ones mask, s * (1 - inpainting_mask_weight).  sdwui conditions a "Latent"
+        second pass with a weight below 1 on the float decode of the upscaled latents: refused.
         Returns uint8 [b, H*hr, W*hr, 3] on device."""
         from . import upscale
         kind, _ = upscale.kind(upscaler)
+        if self.inpainting and kind == "latent" and inpainting_mask_weight < 1:
+            raise ValueError(f"hires upscaler {upscaler!r} with inpainting_mask_weight {inpainting_mask_weight} < 1 is not "
+                             f"served on an inpainting model")
         b = tokens.shape[0]
         h, w = height // 8, width // 8
         h2, w2 = int(height * hr_scale) // 8, int(width * hr_scale) // 8
         if kind != "latent" and (int(height * hr_scale) % 8 or int(width * hr_scale) % 8):
             raise ValueError(f"hires upscaler {upscaler!r}: the target size must be a multiple of 8")
         cond, uncond = self._conds(tokens, neg_tokens, width, height, multipliers, neg_multipliers)
-        lat = self._sample_txt(cond, uncond, seed, b, h, w, steps, cfg_scale, sampler, scheduler, tiling=tiling)
+        lat = self._sample_txt(cond, uncond, seed, b, h, w, steps, cfg_scale, sampler, scheduler, tiling=tiling,
+                               image_cond=self._txt2img_cond(b, h, w, tiling) if self.inpainting else None)
+        image_cond = None
         if kind == "latent":
             with self._ctx():
                 if upscaler == "Latent":
@@ -950,35 +1020,41 @@ class SDEngine:
                 else:
                     up = upscale.resize_latents(lat, upscaler, h, w, h2, w2)
             init = up.reshape(b, h2, w2, 4).permute(0, 3, 1, 2)
+            if self.inpainting:
+                image_cond = self._txt2img_cond(b, h2, w2, tiling)
         else:
             images = self.decode(lat, h, w, tiling)
             f = 2 ** (len(self.vae_cfg.ch_mult) - 1)   # 8 for the kl-f8 autoencoder: the target is then W*hr x H*hr
             with self._ctx():
                 images = upscale.resize_image(images, w2 * f, h2 * f, upscaler, upscaler_tile, upscaler_overlap)
             init = self.encode(images.contiguous(), tiling)
+            if self.inpainting:
+                image_cond = (self.encode_conditioning(images.contiguous(), None, inpainting_mask_weight, tiling), None)
         if self.clip.xl:   # SDXL's vector conditioning carries the target size: the second pass gets its own (sdwui hr_c / hr_uc)
             cond, uncond = self._conds(tokens, neg_tokens, w2 * 8, h2 * 8, multipliers, neg_multipliers)
         lat2 = self._sample_from(init, cond, uncond, seed, denoising_strength, hr_steps or steps, cfg_scale, sampler, scheduler,
-                                 tiling=tiling)
+                                 tiling=tiling, image_cond=image_cond)
         return self.decode(lat2, h2, w2, tiling)
 
     def _sample_txt(self, cond, uncond, seed: int, b: int, h: int, w: int, steps: int, cfg_scale: float, sampler: str,
-                    scheduler: Optional[str], controls=None, tiling: bool = False) -> torch.Tensor:
+                    scheduler: Optional[str], controls=None, tiling: bool = False, image_cond=None) -> torch.Tensor:
         pr = self.program(sampler, scheduler, steps)
         nz = per_image_noise(seed, b, (4, h, w), 1 + pr.draws, *self.variation)
         return self.run_program(cond, uncond, pr.start(nz[0]), pr, cfg_scale, noises=nz[1:] if pr.draws else None,
-                                controls=controls, tiling=tiling)
+                                controls=controls, tiling=tiling, image_cond=image_cond)
 
     @torch.no_grad()
     def txt2img(self, tokens: torch.Tensor, neg_tokens: torch.Tensor, seed: int, steps: int = 20, cfg_scale: float = 7.0,
                 height: int = 512, width: int = 512, sampler: str = "DDIM", scheduler: Optional[str] = None,
                 multipliers: Optional[torch.Tensor] = None, neg_multipliers: Optional[torch.Tensor] = None,
-                controls=None, tiling: bool = False) -> torch.Tensor:
+                controls=None, tiling: bool = False, inpainting_mask_weight: float = 1.0) -> torch.Tensor:
         """Whole request for this engine's share: returns uint8 [b, H, W, 3] on device.  tokens [b, 77 * k] and
         neg_tokens [b, 77 * k'] with their optional emphasis multipliers of the same shapes (factory.tokenize_prompts).
-        `controls`: ControlNet units as for img2img (None: none); `tiling` as for img2img."""
+        `controls`: ControlNet units as for img2img (None: none); `tiling` as for img2img.  An inpainting model gets
+        sdwui's txt2img conditioning, which inpainting_mask_weight does not enter (it is taken for a uniform call)."""
         b = tokens.shape[0]
         h, w = height // 8, width // 8
         cond, uncond = self._conds(tokens, neg_tokens, width, height, multipliers, neg_multipliers)
-        lat = self._sample_txt(cond, uncond, seed, b, h, w, steps, cfg_scale, sampler, scheduler, controls, tiling)
+        lat = self._sample_txt(cond, uncond, seed, b, h, w, steps, cfg_scale, sampler, scheduler, controls, tiling,
+                               self._txt2img_cond(b, h, w, tiling) if self.inpainting else None)
         return self.decode(lat, h, w, tiling)

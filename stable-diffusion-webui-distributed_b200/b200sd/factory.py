@@ -2,10 +2,13 @@
 
 Weights: `SD_CKPT=/path/model.safetensors` (ldm key names; read for sd15 and sd21) when present, otherwise the seeded
 synthetic weights of synth.py (no checkpoint exists offline — every benchmark / parity number in this repo uses those).
-Model family: B200SD_MODEL = sd15 (default) | sdxl | sd21 | tiny | tinyxl | tiny21.  Prediction type: each family's
-default (v for sd21 / tiny21, eps for the others), overridden by B200SD_PREDICTION = eps | v.
+Model family: B200SD_MODEL = sd15 (default) | sdxl | sd21 | tiny | tinyxl | tiny21, each also as an inpainting model with
+a 9-channel UNet (`sd15-inpainting`, ...).  A checkpoint's own conv_in decides between the two: SD_CKPT of an inpainting
+checkpoint serves it as one.  Prediction type: each family's default (v for sd21 / tiny21, eps for the others and for
+every inpainting model, as sdwui's v2-inpainting-inference.yaml), overridden by B200SD_PREDICTION = eps | v.
 ControlNets (controlnet()): B200SD_CONTROLNET_DIR/<model>.safetensors, otherwise seeded synthetic weights.
 """
+import dataclasses
 import logging
 import os
 import threading
@@ -26,6 +29,7 @@ _ENGINES: Dict[str, SDEngine] = {}
 _STATE: Dict[str, Dict[str, torch.Tensor]] = {}
 CKPT_FAMILIES = ("sd15", "sd21")      # families whose weights SD_CKPT replaces (SDXL keeps its synthetic weights)
 V_FAMILIES = ("sd21", "tiny21")       # families served as v-prediction unless B200SD_PREDICTION says otherwise
+INPAINTING = "-inpainting"            # family suffix of the 9-channel inpainting UNets
 
 
 def _load_safetensors(path: str) -> Dict[str, torch.Tensor]:
@@ -38,7 +42,7 @@ def state_dict(size: str = "sd15", seed: int = 0) -> Dict[str, torch.Tensor]:
     with _LOCK:
         if key not in _STATE:
             ckpt = os.environ.get("SD_CKPT")
-            if ckpt and size in CKPT_FAMILIES:
+            if ckpt and _base(size) in CKPT_FAMILIES:
                 _STATE[key] = _load_safetensors(ckpt)
             else:
                 cfgs = configs(size)
@@ -46,7 +50,16 @@ def state_dict(size: str = "sd15", seed: int = 0) -> Dict[str, torch.Tensor]:
         return _STATE[key]
 
 
+def _base(size: str) -> str:
+    """the family without its inpainting suffix"""
+    return size[:-len(INPAINTING)] if size.endswith(INPAINTING) else size
+
+
 def configs(size: str = "sd15"):
+    """(UNet, VAE, text encoder) configs of a family; `<family>-inpainting` is the family's 9-channel UNet"""
+    if size.endswith(INPAINTING):
+        unet, vae, clip = configs(_base(size))
+        return dataclasses.replace(unet, in_channels=9), vae, clip
     if size == "sd15":
         return C.SD15_UNET, C.SD15_VAE, C.SD15_CLIP
     if size == "tiny":
@@ -62,20 +75,32 @@ def configs(size: str = "sd15"):
     raise ValueError(size)
 
 
-def prediction(size: str) -> str:
+def checkpoint_in_channels(sd: Dict[str, torch.Tensor]) -> int:
+    """input channels of a checkpoint's UNet conv_in: 4, 9 for an inpainting model (8 instruct-pix2pix, 5 depth2img)"""
+    return int(sd[C.UNET_PREFIX + "input_blocks.0.0.weight"].shape[1])
+
+
+def prediction(size: str, in_channels: int = 4) -> str:
     """what the family's UNet predicts: B200SD_PREDICTION (eps | v) when set, otherwise v for SD 2.x (768-v), eps for the
-    rest.  SD 2.x-base is B200SD_PREDICTION=eps; v-prediction SD1.5 / SDXL finetunes are B200SD_PREDICTION=v."""
+    rest.  SD 2.x-base is B200SD_PREDICTION=eps; v-prediction SD1.5 / SDXL finetunes are B200SD_PREDICTION=v.  A 9-channel
+    (inpainting) UNet is eps in every family, as sdwui's v2-inpainting-inference.yaml configures 512-inpainting-ema."""
     env = os.environ.get("B200SD_PREDICTION", "").strip()
     if env:
         if env not in ("eps", "v"):
             raise ValueError(f"B200SD_PREDICTION={env!r}: expected 'eps' or 'v'")
         return env
-    return "v" if size in V_FAMILIES else "eps"
+    return "v" if size in V_FAMILIES and in_channels == 4 else "eps"
 
 
 def default_engine_factory(device: str, size: str = None) -> SDEngine:
     size = size or os.environ.get("B200SD_MODEL", "sd15")
-    pred = prediction(size)
+    sd = state_dict(size)
+    unet_cfg, vae_cfg, clip_cfg = configs(size)
+    if os.environ.get("SD_CKPT") and _base(size) in CKPT_FAMILIES:
+        # the checkpoint's conv_in decides: an inpainting checkpoint under a plain family name is served as one, and
+        # 8- / 5-channel models are refused by SDEngine instead of being padded to 64 channels
+        unet_cfg = dataclasses.replace(unet_cfg, in_channels=checkpoint_in_channels(sd))
+    pred = prediction(size, unet_cfg.in_channels)
     key = f"{device}:{size}:{pred}"
     with _LOCK:
         eng = _ENGINES.get(key)
@@ -86,8 +111,8 @@ def default_engine_factory(device: str, size: str = None) -> SDEngine:
         if size != "tiny" and not os.environ.get("SD_TOKENIZER"):
             log.warning("b200sd: SD_TOKENIZER is not set — prompts are hashed to token ids, not BPE-tokenised")
         # SDXL runs in bf16 (BASELINE config 4; its VAE overflows fp16 — sdwui upcasts it, SURVEY App. C)
-        dtype = torch.bfloat16 if size in ("sdxl", "tinyxl") else torch.float16
-        eng = SDEngine(state_dict(size), *configs(size), device=device, dtype=dtype, prediction=pred)
+        dtype = torch.bfloat16 if _base(size) in ("sdxl", "tinyxl") else torch.float16
+        eng = SDEngine(sd, unet_cfg, vae_cfg, clip_cfg, device=device, dtype=dtype, prediction=pred)
         with _LOCK:
             _ENGINES[key] = eng
     return eng
@@ -148,7 +173,7 @@ def model_identity(size: str = None) -> str:
     """what /sd-models and /options report as the loaded checkpoint"""
     size = size or os.environ.get("B200SD_MODEL", "sd15")
     ckpt = os.environ.get("SD_CKPT")
-    return os.path.basename(ckpt) if ckpt and size in CKPT_FAMILIES else f"synthetic-{size}-seed0"
+    return os.path.basename(ckpt) if ckpt and _base(size) in CKPT_FAMILIES else f"synthetic-{size}-seed0"
 
 
 _TOKENIZER = {}

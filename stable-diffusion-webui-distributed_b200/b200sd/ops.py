@@ -366,6 +366,38 @@ def hint_to_nhwc(img_u8: torch.Tensor, out: torch.Tensor):
     return out
 
 
+def masked_image_to_nhwc(img_u8: torch.Tensor, mask_u8: Optional[torch.Tensor], weight: float, out: torch.Tensor):
+    """img_u8 uint8 [B, HW, 3], mask_u8 uint8 [HW] (None: all ones) -> out [B, HW, pitch] channels 0..2 =
+    (2*x/255 - 1) * (1 - weight * [mask >= 128]): an inpainting model's conditioning image"""
+    b, hw, _ = img_u8.shape
+    assert img_u8.dtype == torch.uint8 and img_u8.is_contiguous()
+    assert out.shape[:2] == (b, hw) and out.stride(2) == 1 and out.stride(0) == hw * out.stride(1)
+    assert mask_u8 is None or (mask_u8.dtype == torch.uint8 and mask_u8.is_contiguous() and mask_u8.numel() == hw)
+    rc = _lib.lib().b200sd_masked_image_to_nhwc(_p(img_u8), _p(mask_u8), ctypes.c_float(weight), _p(out),
+                                                ctypes.c_longlong(out.stride(1)), b, hw, _dt(out), _stream())
+    check(rc, "b200sd_masked_image_to_nhwc")
+    _count()
+    return out
+
+
+def pack_image_cond(z: torch.Tensor, mask_u8: Optional[torch.Tensor], xin: torch.Tensor, h: int, w: int):
+    """z fp32 [B, h*w, 4] and the pixel mask uint8 [f*h, f*w] (None: all ones) -> channels 4 (the mask at (f*i, f*j),
+    thresholded at 128) and 5..8 (z) of both [cond | uncond] halves of the UNet input xin [2B, h*w, pitch]"""
+    b = z.shape[0]
+    assert z.dtype == torch.float32 and z.is_contiguous() and z.shape == (b, h * w, 4)
+    assert xin.shape[:2] == (2 * b, h * w) and xin.stride(2) == 1 and xin.stride(0) == h * w * xin.stride(1)
+    f = 1
+    if mask_u8 is not None:
+        f = mask_u8.shape[0] // h
+        assert mask_u8.dtype == torch.uint8 and mask_u8.is_contiguous() and tuple(mask_u8.shape) == (f * h, f * w), \
+            (tuple(mask_u8.shape), h, w)
+    rc = _lib.lib().b200sd_pack_image_cond(_p(z), _p(mask_u8), _p(xin), ctypes.c_longlong(xin.stride(1)), b, h, w, f,
+                                           _dt(xin), _stream())
+    check(rc, "b200sd_pack_image_cond")
+    _count()
+    return xin
+
+
 def unpack_latent(moments: torch.Tensor, x: torch.Tensor, scale: float):
     """moments [B, HW, pitch] (first 4 channels = posterior mean) -> x fp32 [B, HW, 4] = mean * scale"""
     b, hw, _ = moments.shape

@@ -2,7 +2,8 @@
 
 Decoder: stands in for upstream `AutoencoderKL.decode` (ldm/modules/diffusionmodules/model.py::Decoder) + sdwui's
 clamp/255/uint8 conversion — the "final VAE decode" of the north star (SURVEY.md §8 a-ext x11).
-Encoder: `AutoencoderKL.encode(...).mean` (model.py::Encoder + quant_conv) for img2img (§8 a-ext x12); its Downsample
+Encoder: `AutoencoderKL.encode(...).mean` (model.py::Encoder + quant_conv) for img2img (§8 a-ext x12) and for the
+conditioning image of inpainting models (a masked program of its own); its Downsample
 (pad (0,1,0,1), 3x3 stride 2, no padding) is the conv kernel with pad=0 / pad_end=1 and TMA elementStrides=2.
 
 The single-head d=C mid-block attention is expressed with the GEMM kernel: per image S = q k^T, row softmax,
@@ -254,19 +255,37 @@ class VAEDecoderProgram(_VAEProgram):
 
 
 class VAEEncoderProgram(_VAEProgram):
-    """Encode `b` RGB images of size H x W (uint8) -> scaled latents fp32 [b, (H/f)*(W/f), 4] (posterior mean)."""
+    """Encode `b` RGB images of size H x W (uint8) -> scaled latents fp32 [b, (H/f)*(W/f), 4] (posterior mean).
+    masked: the encoded image is an inpainting model's conditioning image s * (1 - weight * [mask >= 128]) of the uint8
+    images, with the mask and weight of set_condition."""
 
-    def __init__(self, w: VAEEncoderWeights, b: int, height: int, width: int, tiling: bool = False):
+    def __init__(self, w: VAEEncoderWeights, b: int, height: int, width: int, tiling: bool = False, masked: bool = False):
         super().__init__(w, b, tiling)
         self.height, self.width = height, width
         self.img_u8 = torch.zeros((b, height * width, 3), device=self.dev, dtype=torch.uint8)
         self.xin = torch.zeros((b, height * width, 64), device=self.dev, dtype=self.dt)  # RGB in channels 0..2
-        self._build()
+        if masked:
+            self.mask_u8 = torch.zeros((height * width,), device=self.dev, dtype=torch.uint8)
+            self.set_condition(None, 1.0)
+        self._build(masked)
         self._finish()
 
-    def _build(self):
+    def set_condition(self, mask_u8, weight: float):
+        """the pixel mask uint8 [H, W] (None: all ones) and inpainting_mask_weight of the next run()s (masked programs)"""
+        if mask_u8 is not None:
+            self.mask_u8.copy_(mask_u8.reshape(-1))
+        self.cond_mask = None if mask_u8 is None else self.mask_u8
+        self.cond_weight = float(weight)
+
+    def _condition_input(self):
+        ops.masked_image_to_nhwc(self.img_u8, self.cond_mask, self.cond_weight, self.xin)
+
+    def _build(self, masked: bool = False):
         b, h, wd, t = self.b, self.height, self.width, self.w.t
-        self._emit(ops.image_to_nhwc, self.img_u8, self.xin)
+        if masked:
+            self._emit(self._condition_input)
+        else:
+            self._emit(ops.image_to_nhwc, self.img_u8, self.xin)
         c = self.w.cfg.ch
         x = self.pool.get(b, h * wd, c)
         emit_conv3(self, self.xin, h, wd, t["conv_in.w"], x, bias=t["conv_in.b"])

@@ -165,6 +165,9 @@ class LocalGPUWorker(Worker):
                     logger.warning(f"scheduler '{scheduler}' is not implemented on worker {self.label}: using the sampler's default")
                 scheduler = None
         controls = self._controls(eng, payload, width, height)
+        # an inpainting checkpoint (9-channel UNet) is conditioned on the mask and the masked init image, with sdwui's
+        # inpainting_mask_weight; other engines never see the setting
+        mask_weight = self._inpainting_mask_weight(payload) if getattr(eng, "inpainting", False) else None
         init_u8 = None
         inpaint = None
         if payload.get("init_images"):
@@ -231,6 +234,8 @@ class LocalGPUWorker(Worker):
         tiling = self._tiling(payload)
         if tiling:     # likewise an untiled payload
             weights["tiling"] = True
+        if mask_weight is not None:
+            weights["inpainting_mask_weight"] = mask_weight
         chunks = []
         for it in range(n_iter):
             # variation seeds: image k of iteration `it` blends noise(seed + k) with noise(subseed + k)
@@ -242,6 +247,8 @@ class LocalGPUWorker(Worker):
                 weights["multipliers"] = mult_all[:batch]
             if init_u8 is not None:
                 kw = {} if inpaint is None else {"latmask": inpaint.latmask, "inpainting_fill": inpaint_fill}
+                if inpaint is not None and mask_weight is not None:   # the conditioning mask: sdwui's image_mask
+                    kw["image_mask"] = torch.from_numpy(np.array(inpaint.fill_mask.convert("L")))
                 u8 = eng.img2img(tok, neg_all, seed_it, init_u8, denoising_strength=denoise, steps=steps,
                                  cfg_scale=cfg_scale, sampler=sampler, scheduler=scheduler, **kw, **weights)
             elif payload.get("enable_hr"):
@@ -289,8 +296,10 @@ class LocalGPUWorker(Worker):
         n = host.shape[0]
         seeds = [seed + (i if strength == 0 else 0) for i in range(n)]
         subseeds = [subseed + i for i in range(n)]
+        # sdwui create_infotext: "Conditional mask weight" when img2img runs with inpainting conditioning
+        cond_weight = f", Conditional mask weight: {mask_weight}" if mask_weight is not None and init_u8 is not None else ""
         infotexts = [f"{prompt}\nNegative prompt: {negative}\nSteps: {steps}, Sampler: {sampler}, CFG scale: {cfg_scale}, "
-                     f"Seed: {s}, Size: {width}x{height}" + (", Tiling: True" if tiling else "") for s in seeds]
+                     f"Seed: {s}, Size: {width}x{height}" + cond_weight + (", Tiling: True" if tiling else "") for s in seeds]
         info = {"all_seeds": seeds, "all_subseeds": subseeds, "all_prompts": [prompt] * n,
                 "all_negative_prompts": [negative] * n, "infotexts": infotexts, "seed": seeds[0], "subseed": subseeds[0],
                 "prompt": prompt, "negative_prompt": negative}
@@ -339,6 +348,19 @@ class LocalGPUWorker(Worker):
             value = getattr(getattr(modules.shared, "opts", None), "tiling", False)
         return bool(value)
 
+    @staticmethod
+    def _inpainting_mask_weight(payload: dict) -> float:
+        """sdwui's inpainting_mask_weight of the request: override_settings, then the options of the sdwui this runs in,
+        then 1.0; outside [0, 1] it is refused"""
+        value = (payload.get("override_settings") or {}).get("inpainting_mask_weight")
+        if value is None:
+            import modules.shared
+            value = getattr(getattr(modules.shared, "opts", None), "inpainting_mask_weight", None)
+        w = 1.0 if value is None else float(value)
+        if not 0.0 <= w <= 1.0:
+            raise ValueError(f"inpainting_mask_weight {w} is outside [0, 1]")
+        return w
+
     def _controls(self, eng, payload: dict, width: int, height: int):
         """the payload's enabled ControlNet units as SDEngine `controls` (None: no unit); refusals raise ValueError"""
         from b200sd import controlnet as ctl, factory
@@ -347,6 +369,8 @@ class LocalGPUWorker(Worker):
             return None
         if eng.unet_cfg.adm_in_channels:
             raise ValueError("ControlNet is not served for SDXL")
+        if getattr(eng, "inpainting", False):
+            raise ValueError("ControlNet is not served with an inpainting checkpoint")
         if payload.get("enable_hr") and not payload.get("init_images"):
             raise ValueError("ControlNet together with the hires fix is not served")
         return [(factory.controlnet(u.model, device=str(eng.device), dtype=eng.dtype), u.image, u.weight, u.start, u.end)
