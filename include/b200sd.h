@@ -256,6 +256,31 @@ int b200sd_scaled_add(const void* X, long long pitch_x, void* Y, long long pitch
  * timestep samplers, and once more after sampling) */
 int b200sd_blend_latent(float* x, const float* init, const float* latmask, int B, int HW, void* stream);
 
+/* ---- token merging (tomesd bipartite soft matching on the 2x2 grid, as sdwui's token_merging_ratio applies it to the
+ * self-attention of the UNet's full-resolution transformer blocks).  fp16 only: bf16 is B200SD_ERR_UNSUPPORTED.
+ * Tokens of a batch row are the H*W latent pixels t = y*W + x (H, W even); the top-left token of every 2x2 block is a
+ * dst token (index j = (y/2)*(W/2) + x/2), the other Ns = 3/4 N are src tokens, numbered in ascending token order.
+ * A merged sequence of Nm = N - r slots: slots [0, Ns - r) are the unmerged src tokens in ascending token order, slot
+ * Ns - r + j is dst token j with the src tokens merged into it. */
+/* bytes of the caller-owned workspace b200sd_tome_match takes (-1: unsupported shape; C must be 64 or 320) */
+long long b200sd_tome_match_workspace_bytes(int B, int H, int W, int C);
+/* matching of X [B,H*W,C] (row pitch `pitch`), per batch row: metric = X / ||X|| rounded to fp16; for every src token
+ * a, node_max / node_idx = max / argmax over dst b of metric_a . metric_b (fp32 accumulation, ties to the lowest dst
+ * index; a fused wgmma kernel, no score matrix is stored); the r src tokens with the largest (node_max desc, src index
+ * asc) keys are merged into their node_idx dst (1 <= r <= Ns).  Outputs int32: slot [B][N] (the slot of every token),
+ * members [B][N] (tokens ordered by slot, ascending within a slot), seg [B][Nm+1] (slot s holds members[seg[s] ..
+ * seg[s+1])). */
+int b200sd_tome_match(const void* X, long long pitch, int B, int H, int W, int C, int r, int* slot, int* members,
+                      int* seg, void* workspace, long long workspace_bytes, int dtype, void* stream);
+/* Y[b,s,:] = mean of X[b,t,:] over the members t of slot s: fp32 sum in ascending token order, divided by the count and
+ * rounded once (tomesd merge: scatter_reduce "mean", include_self).  X [B,N,C], Y [B,Nm,C]; C % 8 == 0. */
+int b200sd_tome_merge(const void* X, long long pitch_x, const int* members, const int* seg, void* Y, long long pitch_y,
+                      int B, int N, int Nm, int C, int dtype, void* stream);
+/* out[b,t,:] = round(R[b,t,:] + Y[b, slot[b,t], :]) (tomesd unmerge, then the block's residual add).  R, out [B,N,C],
+ * Y [B,Nm,C]. */
+int b200sd_tome_unmerge_add(const void* R, long long pitch_r, const void* Y, long long pitch_y, const int* slot,
+                            void* out, long long pitch_o, int B, int N, int Nm, int C, int dtype, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

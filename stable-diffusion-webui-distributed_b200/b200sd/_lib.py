@@ -53,6 +53,7 @@ def load(path: str = LIB_PATH) -> ctypes.CDLL:
             raise B200SDError(f"{path} does not export {name}")
     lib.b200sd_version.restype = ctypes.c_char_p
     lib.b200sd_groupnorm_stats_floats.restype = ctypes.c_longlong
+    lib.b200sd_tome_match_workspace_bytes.restype = ctypes.c_longlong
     return lib
 
 

@@ -262,12 +262,14 @@ class Program:
 # ------------------------------------------------------------------------------------------------ plans
 class Plan:
     """Everything shape-dependent for (images per call b, latent h x w) on one device.  tiling: the UNet's and the VAE
-    decoder's 3x3 convs pad circularly (sdwui's tiling option)."""
+    decoder's 3x3 convs pad circularly (sdwui's tiling option).  token_merging: r tokens merged in the UNet's
+    full-resolution self-attention (sdwui's token merging ratio, SDEngine.merged_tokens)."""
 
-    def __init__(self, eng: "SDEngine", b: int, h: int, w: int, vae_chunk: int, tiling: bool = False):
+    def __init__(self, eng: "SDEngine", b: int, h: int, w: int, vae_chunk: int, tiling: bool = False,
+                 token_merging: int = 0):
         dev = eng.device
         self.b, self.h, self.w = b, h, w
-        self.unet = UNetProgram(eng.unet_w, 2 * b, h, w, CHUNK, tiling=tiling)
+        self.unet = UNetProgram(eng.unet_w, 2 * b, h, w, CHUNK, tiling=tiling, token_merging=token_merging)
         self.kv_len = self.unet.kv_len   # int32 [2b] on the device: context tokens of every [cond | uncond] row
         self.vae_chunk = min(vae_chunk, b)
         self.vae = VAEDecoderProgram(eng.vae_w, self.vae_chunk, h, w, tiling=tiling)
@@ -459,9 +461,22 @@ class SDEngine:
             self._cap_stream = torch.cuda.Stream(device=self.device)
         return self._cap_stream
 
-    def plan(self, b: int, h: int, w: int, tiling: bool = False) -> Plan:
-        """the plan of (b, h, w); tiled plans are kept apart under (b, h, w, "tiling")"""
+    def merged_tokens(self, h: int, w: int, ratio: float) -> int:
+        """r of sdwui's token merging at `ratio` for an h x w latent: tomesd's int(N * ratio) of the N = h*w tokens of the
+        full-resolution transformer blocks, capped at the 3/4 N src tokens of the 2x2 grid.  0 for a ratio <= 0 (sdwui
+        patches nothing) and for a UNet without attention at full resolution (SDXL)."""
+        if not ratio > 0 or not self.unet_cfg.depth(0):
+            return 0
+        n = h * w
+        return min(n - (h // 2) * (w // 2), int(n * ratio))
+
+    def plan(self, b: int, h: int, w: int, tiling: bool = False, token_merging_ratio: float = 0.0) -> Plan:
+        """the plan of (b, h, w); tiled plans are kept apart under (b, h, w, "tiling"), and plans that merge r > 0 tokens
+        under the same key + ("tome", r)"""
+        r = self.merged_tokens(h, w, token_merging_ratio)
         key = (b, h, w, "tiling") if tiling else (b, h, w)
+        if r:
+            key += ("tome", r)
         down = 2 ** (len(self.unet_cfg.channel_mult) - 1)
         if b < 1 or h < down or w < down or h % down or w % down:
             # the UNet halves the latent len(channel_mult) - 1 times and concatenates skip tensors on the way up: upstream
@@ -473,7 +488,7 @@ class SDEngine:
                 old = self.plans.pop(next(iter(self.plans)))
                 old.graphs.clear()
             with self._ctx():
-                self.plans[key] = Plan(self, b, h, w, self.vae_chunk, tiling)
+                self.plans[key] = Plan(self, b, h, w, self.vae_chunk, tiling, r)
         else:
             self.plans[key] = self.plans.pop(key)   # most recently used last
         return self.plans[key]
@@ -650,14 +665,15 @@ class SDEngine:
     @torch.no_grad()
     def run_program(self, cond: torch.Tensor, uncond: torch.Tensor, x_start: torch.Tensor, pr: "Program", cfg_scale: float,
                     noises: Optional[torch.Tensor] = None, inpaint=None, controls=None,
-                    tiling: bool = False, image_cond=None) -> torch.Tensor:
+                    tiling: bool = False, image_cond=None, token_merging_ratio: float = 0.0) -> torch.Tensor:
         """cond/uncond [b, 77 * k, ctx] on device (cond and uncond may have different k); x_start [b, 4, h, w] fp32 (host or device) = Program.start(...): the start
         latents in the sampler's own space; noises [pr.draws, b, 4, h, w]: the per-image N(0,1) draws after the first;
         inpaint = (clean init latents [b, 4, h, w], latent mask [h * w]).  controls: ControlNet units, see _set_controls
         (None: no ControlNet).  tiling: the UNet's convs pad circularly (its own plan).  image_cond = (masked-image
         latents fp32 [b, 4, h, w], pixel mask uint8 [f*h, f*w] or None for all ones): an inpainting model's extra UNet
-        input channels, packed once before sampling (required for a 9-channel UNet, refused for a 4-channel one).  Returns
-        the final latents fp32 [b, h*w, 4] (NHWC, a view of plan state)."""
+        input channels, packed once before sampling (required for a 9-channel UNet, refused for a 4-channel one).
+        token_merging_ratio: sdwui's token merging (its own plan; see merged_tokens).  Returns the final latents fp32
+        [b, h*w, 4] (NHWC, a view of plan state)."""
         b, _, h, w = x_start.shape
         if pr.draws and (noises is None or noises.shape[0] < pr.draws):
             raise ValueError(f"{pr.sampler} needs {pr.draws} per-image noise draws")
@@ -670,7 +686,7 @@ class SDEngine:
         cond = cond if isinstance(cond, Cond) else Cond(cond)
         uncond = uncond if isinstance(uncond, Cond) else Cond(uncond)
         with self._ctx():
-            plan = self.plan(b, h, w, tiling)
+            plan = self.plan(b, h, w, tiling, token_merging_ratio)
             if controls and cond.y is not None:
                 raise ValueError("ControlNet is not served for SDXL")
             self._windows = self._set_controls(plan, controls) if controls else []
@@ -839,12 +855,14 @@ class SDEngine:
         return self.run_program(cond, uncond, x_T.to(torch.float32) * pr.noise_scale, pr, cfg_scale, noises, inpaint)
 
     @torch.no_grad()
-    def decode(self, latents: torch.Tensor, h: int, w: int, tiling: bool = False) -> torch.Tensor:
+    def decode(self, latents: torch.Tensor, h: int, w: int, tiling: bool = False,
+               token_merging_ratio: float = 0.0) -> torch.Tensor:
         """latents fp32 [b, h*w, 4] (scaled) -> uint8 [b, 8h, 8w, 3] on device.  tiling: circular convs (the tiled plan's
-        decoder)."""
+        decoder).  token_merging_ratio: the decoder of the plan that sampled them (merging does not touch the VAE; the
+        request then builds one plan, not two)."""
         b = latents.shape[0]
         with self._ctx():
-            plan = self.plan(b, h, w, tiling)
+            plan = self.plan(b, h, w, tiling, token_merging_ratio)
             vae = plan.vae
             out = torch.empty((b, vae.out_h * vae.out_w, 3), device=self.device, dtype=torch.uint8)
             c = plan.vae_chunk
@@ -921,7 +939,8 @@ class SDEngine:
                 scheduler: Optional[str] = None, latmask: Optional[torch.Tensor] = None,
                 inpainting_fill: int = 1, multipliers: Optional[torch.Tensor] = None,
                 neg_multipliers: Optional[torch.Tensor] = None, controls=None, tiling: bool = False,
-                image_mask: Optional[torch.Tensor] = None, inpainting_mask_weight: float = 1.0) -> torch.Tensor:
+                image_mask: Optional[torch.Tensor] = None, inpainting_mask_weight: float = 1.0,
+                token_merging_ratio: float = 0.0) -> torch.Tensor:
         """img2img: VAE-encode the init images (posterior mean), noise them to t_enc, run the remaining part of the
         sampler's schedule, decode.  init_u8 uint8 [b, H, W, 3].  Returns uint8 [b, H, W, 3] on device.
         `latmask` fp32 [h * w] (b200sd.inpaint.prepare_mask): inpainting — the region with latmask 0 is held to the init
@@ -938,7 +957,9 @@ class SDEngine:
         Inpainting models (9 input channels) are conditioned on the mask and the VAE latents of
         init * (1 - inpainting_mask_weight * mask) (sdwui img2img_image_conditioning): `image_mask` uint8 [H, W] is the
         processed pixel mask (inpaint.InpaintMask.fill_mask), required with `latmask`; without a mask it is all ones.
-        Other models ignore both arguments."""
+        Other models ignore both arguments.
+        `token_merging_ratio`: sdwui's token merging (tomesd) in the UNet's full-resolution self-attention; <= 0 does not
+        merge."""
         b = tokens.shape[0]
         cond, uncond = self._conds(tokens, neg_tokens, init_u8.shape[2], init_u8.shape[1], multipliers, neg_multipliers)
         init = self.encode(init_u8, tiling)
@@ -955,8 +976,8 @@ class SDEngine:
                 init = init + per_image_noise(seed, b, (4, h, w), 1, *self.variation)[0].to(self.device) * nm
         lat = self._sample_from(init, cond, uncond, seed, denoising_strength, steps, cfg_scale, sampler, scheduler,
                                 inpaint=None if latmask is None else (init, latmask), controls=controls, tiling=tiling,
-                                image_cond=image_cond)
-        return self.decode(lat, h, w, tiling)
+                                image_cond=image_cond, token_merging_ratio=token_merging_ratio)
+        return self.decode(lat, h, w, tiling, token_merging_ratio)
 
     def _txt2img_cond(self, b: int, h: int, w: int, tiling: bool):
         """sdwui txt2img_image_conditioning of an inpainting model at latent size h x w: an all-ones mask over a gray image
@@ -968,7 +989,7 @@ class SDEngine:
 
     def _sample_from(self, init: torch.Tensor, cond, uncond, seed: int, denoising_strength: float, steps: int,
                      cfg_scale: float, sampler: str, scheduler: Optional[str], inpaint=None, controls=None,
-                     tiling: bool = False, image_cond=None) -> torch.Tensor:
+                     tiling: bool = False, image_cond=None, token_merging_ratio: float = 0.0) -> torch.Tensor:
         """the img2img half of a sampler (also the second pass of the hires fix): `init` [b, 4, h, w] latents on the device,
         fresh per-image noise from `seed`, start at the noise level of t_enc.
         DDIM / PLMS: sdwui sd_samplers_timesteps.sample_img2img; k-diffusion samplers: KDiffusionSampler.sample_img2img."""
@@ -977,7 +998,7 @@ class SDEngine:
         nz = per_image_noise(seed, b, (4, h, w), 1 + pr.draws, *self.variation)
         return self.run_program(cond, uncond, pr.start(nz[0].to(self.device), init), pr, cfg_scale,
                                 noises=nz[1:] if pr.draws else None, inpaint=inpaint, controls=controls, tiling=tiling,
-                                image_cond=image_cond)
+                                image_cond=image_cond, token_merging_ratio=token_merging_ratio)
 
     @torch.no_grad()
     def txt2img_hires(self, tokens: torch.Tensor, neg_tokens: torch.Tensor, seed: int, steps: int = 20,
@@ -986,7 +1007,8 @@ class SDEngine:
                       scheduler: Optional[str] = None, multipliers: Optional[torch.Tensor] = None,
                       neg_multipliers: Optional[torch.Tensor] = None, upscaler: str = "Latent",
                       upscaler_tile: int = 192, upscaler_overlap: int = 8, tiling: bool = False,
-                      inpainting_mask_weight: float = 1.0) -> torch.Tensor:
+                      inpainting_mask_weight: float = 1.0, token_merging_ratio: float = 0.0,
+                      token_merging_ratio_hr: float = 0.0) -> torch.Tensor:
         """txt2img with sdwui's hires fix (StableDiffusionProcessingTxt2Img.sample / sample_hr_pass): first pass at
         (height, width), the `upscaler` to hr_scale x, a fresh per-image noise of the large shape from the same seeds,
         then the same sampler's img2img half from t_enc with `hr_steps` (0 = `steps`) steps, decode at the large size.
@@ -997,6 +1019,7 @@ class SDEngine:
         Inpainting models: the first pass and a "Latent" second pass get txt2img's conditioning, a pixel upscaler's second
         pass the upscaled images' under an all-ones mask, s * (1 - inpainting_mask_weight).  sdwui conditions a "Latent"
         second pass with a weight below 1 on the float decode of the upscaled latents: refused.
+        Token merging: the first pass (and its decode) at `token_merging_ratio`, the second at `token_merging_ratio_hr`.
         Returns uint8 [b, H*hr, W*hr, 3] on device."""
         from . import upscale
         kind, _ = upscale.kind(upscaler)
@@ -1010,7 +1033,8 @@ class SDEngine:
             raise ValueError(f"hires upscaler {upscaler!r}: the target size must be a multiple of 8")
         cond, uncond = self._conds(tokens, neg_tokens, width, height, multipliers, neg_multipliers)
         lat = self._sample_txt(cond, uncond, seed, b, h, w, steps, cfg_scale, sampler, scheduler, tiling=tiling,
-                               image_cond=self._txt2img_cond(b, h, w, tiling) if self.inpainting else None)
+                               image_cond=self._txt2img_cond(b, h, w, tiling) if self.inpainting else None,
+                               token_merging_ratio=token_merging_ratio)
         image_cond = None
         if kind == "latent":
             with self._ctx():
@@ -1023,7 +1047,7 @@ class SDEngine:
             if self.inpainting:
                 image_cond = self._txt2img_cond(b, h2, w2, tiling)
         else:
-            images = self.decode(lat, h, w, tiling)
+            images = self.decode(lat, h, w, tiling, token_merging_ratio)
             f = 2 ** (len(self.vae_cfg.ch_mult) - 1)   # 8 for the kl-f8 autoencoder: the target is then W*hr x H*hr
             with self._ctx():
                 images = upscale.resize_image(images, w2 * f, h2 * f, upscaler, upscaler_tile, upscaler_overlap)
@@ -1033,28 +1057,32 @@ class SDEngine:
         if self.clip.xl:   # SDXL's vector conditioning carries the target size: the second pass gets its own (sdwui hr_c / hr_uc)
             cond, uncond = self._conds(tokens, neg_tokens, w2 * 8, h2 * 8, multipliers, neg_multipliers)
         lat2 = self._sample_from(init, cond, uncond, seed, denoising_strength, hr_steps or steps, cfg_scale, sampler, scheduler,
-                                 tiling=tiling, image_cond=image_cond)
-        return self.decode(lat2, h2, w2, tiling)
+                                 tiling=tiling, image_cond=image_cond, token_merging_ratio=token_merging_ratio_hr)
+        return self.decode(lat2, h2, w2, tiling, token_merging_ratio_hr)
 
     def _sample_txt(self, cond, uncond, seed: int, b: int, h: int, w: int, steps: int, cfg_scale: float, sampler: str,
-                    scheduler: Optional[str], controls=None, tiling: bool = False, image_cond=None) -> torch.Tensor:
+                    scheduler: Optional[str], controls=None, tiling: bool = False, image_cond=None,
+                    token_merging_ratio: float = 0.0) -> torch.Tensor:
         pr = self.program(sampler, scheduler, steps)
         nz = per_image_noise(seed, b, (4, h, w), 1 + pr.draws, *self.variation)
         return self.run_program(cond, uncond, pr.start(nz[0]), pr, cfg_scale, noises=nz[1:] if pr.draws else None,
-                                controls=controls, tiling=tiling, image_cond=image_cond)
+                                controls=controls, tiling=tiling, image_cond=image_cond,
+                                token_merging_ratio=token_merging_ratio)
 
     @torch.no_grad()
     def txt2img(self, tokens: torch.Tensor, neg_tokens: torch.Tensor, seed: int, steps: int = 20, cfg_scale: float = 7.0,
                 height: int = 512, width: int = 512, sampler: str = "DDIM", scheduler: Optional[str] = None,
                 multipliers: Optional[torch.Tensor] = None, neg_multipliers: Optional[torch.Tensor] = None,
-                controls=None, tiling: bool = False, inpainting_mask_weight: float = 1.0) -> torch.Tensor:
+                controls=None, tiling: bool = False, inpainting_mask_weight: float = 1.0,
+                token_merging_ratio: float = 0.0) -> torch.Tensor:
         """Whole request for this engine's share: returns uint8 [b, H, W, 3] on device.  tokens [b, 77 * k] and
         neg_tokens [b, 77 * k'] with their optional emphasis multipliers of the same shapes (factory.tokenize_prompts).
         `controls`: ControlNet units as for img2img (None: none); `tiling` as for img2img.  An inpainting model gets
-        sdwui's txt2img conditioning, which inpainting_mask_weight does not enter (it is taken for a uniform call)."""
+        sdwui's txt2img conditioning, which inpainting_mask_weight does not enter (it is taken for a uniform call).
+        `token_merging_ratio` as for img2img."""
         b = tokens.shape[0]
         h, w = height // 8, width // 8
         cond, uncond = self._conds(tokens, neg_tokens, width, height, multipliers, neg_multipliers)
         lat = self._sample_txt(cond, uncond, seed, b, h, w, steps, cfg_scale, sampler, scheduler, controls, tiling,
-                               self._txt2img_cond(b, h, w, tiling) if self.inpainting else None)
-        return self.decode(lat, h, w, tiling)
+                               self._txt2img_cond(b, h, w, tiling) if self.inpainting else None, token_merging_ratio)
+        return self.decode(lat, h, w, tiling, token_merging_ratio)

@@ -566,3 +566,63 @@ def resize_latent_table(x: torch.Tensor, y: torch.Tensor, h: int, w: int, ho: in
     check(rc, "b200sd_resize_latent_table")
     _count()
     return y
+
+
+# ---- token merging (tomesd as sdwui's token_merging_ratio applies it; b200sd_tome_*)
+_TOME_WS = {}
+
+
+def tome_workspace_bytes(nb: int, h: int, w: int, c: int) -> int:
+    """bytes of the caller-owned workspace tome_match needs for [nb, h*w, c] (C 64 or 320, h and w even)"""
+    key = (nb, h, w, c)
+    n = _TOME_WS.get(key)
+    if n is None:
+        n = int(_lib.lib().b200sd_tome_match_workspace_bytes(nb, h, w, c))
+        if n < 0:
+            raise _lib.B200SDError(f"tome_match: unsupported shape {h}x{w} C={c}")
+        _TOME_WS[key] = n
+    return n
+
+
+def tome_match(x: torch.Tensor, h: int, w: int, r: int, slot: torch.Tensor, members: torch.Tensor, seg: torch.Tensor,
+               workspace: torch.Tensor):
+    """x [NB, h*w, C] fp16 (pitch = stride(1)): the matching of r merged tokens per row -> slot [NB, h*w],
+    members [NB, h*w], seg [NB, h*w - r + 1] int32 (include/b200sd.h)"""
+    nb, n, c = x.shape
+    assert n == h * w and x.stride(2) == 1 and x.stride(0) == n * x.stride(1)
+    for t, cols in ((slot, n), (members, n), (seg, n - r + 1)):
+        assert t.dtype == torch.int32 and t.is_contiguous() and tuple(t.shape) == (nb, cols), (tuple(t.shape), cols)
+    assert workspace.dtype == torch.uint8 and workspace.is_contiguous()
+    rc = _lib.lib().b200sd_tome_match(_p(x), ctypes.c_longlong(x.stride(1)), nb, h, w, c, r, _p(slot), _p(members),
+                                      _p(seg), _p(workspace), ctypes.c_longlong(workspace.numel()), _dt(x), _stream())
+    check(rc, f"b200sd_tome_match NB={nb} H={h} W={w} C={c} r={r}")
+    _count(3)
+
+
+def tome_merge(x: torch.Tensor, members: torch.Tensor, seg: torch.Tensor, out: torch.Tensor):
+    """out [NB, Nm, C] = fp32 mean of x [NB, N, C] over every slot's members"""
+    nb, n, c = x.shape
+    nm = out.shape[1]
+    for t in (x, out):
+        assert t.stride(2) == 1 and t.stride(0) == t.shape[1] * t.stride(1)
+    assert out.shape == (nb, nm, c) and seg.shape == (nb, nm + 1) and members.shape == (nb, n)
+    rc = _lib.lib().b200sd_tome_merge(_p(x), ctypes.c_longlong(x.stride(1)), _p(members), _p(seg), _p(out),
+                                      ctypes.c_longlong(out.stride(1)), nb, n, nm, c, _dt(x), _stream())
+    check(rc, f"b200sd_tome_merge NB={nb} N={n} Nm={nm} C={c}")
+    _count()
+    return out
+
+
+def tome_unmerge_add(residual: torch.Tensor, y: torch.Tensor, slot: torch.Tensor, out: torch.Tensor):
+    """out [NB, N, C] = residual + y[slot] (y [NB, Nm, C], the merged rows' block output)"""
+    nb, n, c = residual.shape
+    nm = y.shape[1]
+    for t in (residual, y, out):
+        assert t.stride(2) == 1 and t.stride(0) == t.shape[1] * t.stride(1)
+    assert out.shape == residual.shape and y.shape == (nb, nm, c) and slot.shape == (nb, n)
+    rc = _lib.lib().b200sd_tome_unmerge_add(_p(residual), ctypes.c_longlong(residual.stride(1)), _p(y),
+                                            ctypes.c_longlong(y.stride(1)), _p(slot), _p(out),
+                                            ctypes.c_longlong(out.stride(1)), nb, n, nm, c, _dt(y), _stream())
+    check(rc, f"b200sd_tome_unmerge_add NB={nb} N={n} Nm={nm} C={c}")
+    _count()
+    return out

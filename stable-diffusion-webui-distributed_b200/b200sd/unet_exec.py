@@ -243,10 +243,18 @@ class ControlNetWeights(UNetWeights):
 class UNetProgram:
     """One UNet evaluation for a fixed (N, H, W): `run()` launches ~700 kernels, no allocation, no sync."""
 
-    def __init__(self, w: UNetWeights, n: int, h: int, wd: int, ctx_len: int = 77, tiling: bool = False):
-        """tiling: every 3x3 conv of the UNet pads circularly (sdwui's tiling option); ControlNet segments never do"""
+    def __init__(self, w: UNetWeights, n: int, h: int, wd: int, ctx_len: int = 77, tiling: bool = False,
+                 token_merging: int = 0):
+        """tiling: every 3x3 conv of the UNet pads circularly (sdwui's tiling option); ControlNet segments never do.
+        token_merging: r > 0 merges r of the h*wd tokens before the self-attention of every transformer block at the full
+        latent resolution (tomesd as sdwui's token_merging_ratio applies it); ControlNet segments never merge."""
         self.w, self.cfg = w, w.cfg
         self.tiling = self.circular = tiling
+        self.token_merging = self.merging = token_merging
+        # per merging transformer block: the matching of the last evaluation, int32 (slot [n, h*wd], members [n, h*wd],
+        # seg [n, h*wd - r + 1]; include/b200sd.h b200sd_tome_match), persistent like kv_len
+        self.tome: Dict[str, tuple] = {}
+        self.tome_ws: Optional[torch.Tensor] = None   # b200sd_tome_match's workspace, shared by those blocks
         self.n, self.h, self.wd = n, h, wd
         self.dev, self.dt = w.device, w.dtype
         self.pool = Pool(self.dev, self.dt)
@@ -337,14 +345,17 @@ class UNetProgram:
         saved = (self.w, self.cur_bias, self.ctx_kv, self._xattn, self.ops, self.op_flops, self.gn_elems, self.ln_elems)
         self.w, self.cur_bias, self.ctx_kv, self._xattn, self.ops, self.op_flops = \
             seg.w, seg.cur_bias, seg.ctx_kv, seg.xattn, seg.ops, seg.op_flops
-        # sd-webui-controlnet's model is not part of the sd model that sdwui's tiling makes circular: zero padding
+        # sd-webui-controlnet's model is not part of the sd model that sdwui's tiling makes circular and tomesd
+        # patches: zero padding, no merging
         self.circular = False
+        self.merging = 0
         try:
             yield
         finally:
             (self.w, self.cur_bias, self.ctx_kv, self._xattn, self.ops, self.op_flops, self.gn_elems,
              self.ln_elems) = saved
             self.circular = self.tiling
+            self.merging = self.token_merging
 
     def _run_layers(self, prefix, layers, x, h, wd, final_dest, conv_in_residual=None):
         """x: input view; the LAST layer writes into final_dest (a view with the right channel count).  conv_in reads the
@@ -441,15 +452,19 @@ class UNetProgram:
             self.ln_elems += 3 * n * hw * c
             # --- self attention
             self._emit(ops.layernorm, hcur, a, t[tb + ".norm1.g"], t[tb + ".norm1.beta"], 1e-5)
-            qkv = self.pool.get(n, hw, 3 * heads * dp)
-            self._emit(ops.linear, a, t[tb + ".attn1.qkv.w"], qkv, bias=t[tb + ".attn1.qkv.b"],
-                       algo_flops=2.0 * n * hw * 3 * c * c)
-            q, k, v = (qkv[..., j * heads * dp:(j + 1) * heads * dp] for j in range(3))
-            o = self.pool.get(n, hw, c)
-            self._emit(ops.attention, q, k, v, o, heads, d, dp, scale, dp > d)
-            self.pool.put(qkv)
-            h1 = self.pool.get(n, hw, c)
-            self._emit(ops.linear, o, t[tb + ".attn1.out.w"], h1, bias=t[tb + ".attn1.out.b"], residual=hcur)
+            if self.merging and (h, wd) == (self.h, self.wd):
+                h1 = self._merged_self_attention(tb, hcur, a, h, wd, c, heads, d, dp, scale)
+                o = self.pool.get(n, hw, c)
+            else:
+                qkv = self.pool.get(n, hw, 3 * heads * dp)
+                self._emit(ops.linear, a, t[tb + ".attn1.qkv.w"], qkv, bias=t[tb + ".attn1.qkv.b"],
+                           algo_flops=2.0 * n * hw * 3 * c * c)
+                q, k, v = (qkv[..., j * heads * dp:(j + 1) * heads * dp] for j in range(3))
+                o = self.pool.get(n, hw, c)
+                self._emit(ops.attention, q, k, v, o, heads, d, dp, scale, dp > d)
+                self.pool.put(qkv)
+                h1 = self.pool.get(n, hw, c)
+                self._emit(ops.linear, o, t[tb + ".attn1.out.w"], h1, bias=t[tb + ".attn1.out.b"], residual=hcur)
             self.pool.put(hcur)
             # --- cross attention (K/V of the context are precomputed per request)
             self._emit(ops.layernorm, h1, a, t[tb + ".norm2.g"], t[tb + ".norm2.beta"], 1e-5)
@@ -475,6 +490,35 @@ class UNetProgram:
         self._emit(ops.linear, hcur, t[key + ".proj_out.w"], dest, bias=t[key + ".proj_out.b"], residual=x)
         self.pool.put(hcur)
         self.pool.put(a)
+
+    def _merged_self_attention(self, tb, hcur, a, h, wd, c, heads, d, dp, scale):
+        """tomesd's ToMeBlock self-attention, u(attn1(m(norm1(x)))) + x: match on the block input hcur, merge the
+        LayerNorm output `a` into h*wd - r rows, q/k/v projection, attention and out-projection on those rows, then
+        give every token its slot's row plus its residual.  Returns h1 [n, h*wd, c] (pool)."""
+        n, hw, t, r = self.n, h * wd, self.w.t, self.merging
+        nm = hw - r
+        if self.tome_ws is None:
+            self.tome_ws = torch.zeros((ops.tome_workspace_bytes(n, h, wd, c),), device=self.dev, dtype=torch.uint8)
+        slot, members, seg = self.tome[tb] = tuple(torch.zeros((n, cols), device=self.dev, dtype=torch.int32)
+                                                   for cols in (hw, hw, nm + 1))
+        self._emit(ops.tome_match, hcur, h, wd, r, slot, members, seg, self.tome_ws)
+        am = self.pool.get(n, nm, c)
+        self._emit(ops.tome_merge, a, members, seg, am)
+        qkv = self.pool.get(n, nm, 3 * heads * dp)
+        self._emit(ops.linear, am, t[tb + ".attn1.qkv.w"], qkv, bias=t[tb + ".attn1.qkv.b"],
+                   algo_flops=2.0 * n * nm * 3 * c * c)
+        self.pool.put(am)
+        q, k, v = (qkv[..., j * heads * dp:(j + 1) * heads * dp] for j in range(3))
+        om = self.pool.get(n, nm, c)
+        self._emit(ops.attention, q, k, v, om, heads, d, dp, scale, dp > d)
+        self.pool.put(qkv)
+        y = self.pool.get(n, nm, c)
+        self._emit(ops.linear, om, t[tb + ".attn1.out.w"], y, bias=t[tb + ".attn1.out.b"])
+        self.pool.put(om)
+        h1 = self.pool.get(n, hw, c)
+        self._emit(ops.tome_unmerge_add, hcur, y, slot, h1)
+        self.pool.put(y)
+        return h1
 
     def _build(self):
         cfg, n, t = self.cfg, self.n, self.w.t

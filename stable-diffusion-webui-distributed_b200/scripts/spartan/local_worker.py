@@ -236,6 +236,10 @@ class LocalGPUWorker(Worker):
             weights["tiling"] = True
         if mask_weight is not None:
             weights["inpainting_mask_weight"] = mask_weight
+        tome, tome_hr = self._token_merging(payload, img2img=init_u8 is not None)
+        # a payload whose ratio resolves to 0 (or below: nothing is merged) reaches the engine with exactly the
+        # arguments it always had
+        tome_kw = {"token_merging_ratio": float(tome)} if tome > 0 else {}
         chunks = []
         for it in range(n_iter):
             # variation seeds: image k of iteration `it` blends noise(seed + k) with noise(subseed + k)
@@ -250,13 +254,15 @@ class LocalGPUWorker(Worker):
                 if inpaint is not None and mask_weight is not None:   # the conditioning mask: sdwui's image_mask
                     kw["image_mask"] = torch.from_numpy(np.array(inpaint.fill_mask.convert("L")))
                 u8 = eng.img2img(tok, neg_all, seed_it, init_u8, denoising_strength=denoise, steps=steps,
-                                 cfg_scale=cfg_scale, sampler=sampler, scheduler=scheduler, **kw, **weights)
+                                 cfg_scale=cfg_scale, sampler=sampler, scheduler=scheduler, **kw, **weights, **tome_kw)
             elif payload.get("enable_hr"):
                 # hires fix (reference eta_hr, worker.py:205): second pass at hr_scale x after the hr_upscaler
                 hr_scale = float(payload.get("hr_scale") or 2.0)
                 if payload.get("hr_resize_x") and payload.get("hr_resize_y"):
                     hr_scale = float(payload["hr_resize_x"]) / width
-                hires = dict(weights)
+                hires = dict(weights, **tome_kw)
+                if tome_hr > 0:
+                    hires["token_merging_ratio_hr"] = float(tome_hr)
                 hires.update(self._hires_upscaler(payload, width, height, hr_scale))
                 u8 = eng.txt2img_hires(tok, neg_all, seed_it, steps=steps, cfg_scale=cfg_scale, height=height,
                                        width=width, hr_scale=hr_scale,
@@ -265,7 +271,7 @@ class LocalGPUWorker(Worker):
                                        scheduler=scheduler, **hires)
             else:
                 u8 = eng.txt2img(tok, neg_all, seed_it, steps=steps, cfg_scale=cfg_scale, height=height,
-                                 width=width, sampler=sampler, scheduler=scheduler, **weights)
+                                 width=width, sampler=sampler, scheduler=scheduler, **weights, **tome_kw)
             chunks.append(u8)
             if eng.interrupted:
                 break
@@ -298,6 +304,11 @@ class LocalGPUWorker(Worker):
         subseeds = [subseed + i for i in range(n)]
         # sdwui create_infotext: "Conditional mask weight" when img2img runs with inpainting conditioning
         cond_weight = f", Conditional mask weight: {mask_weight}" if mask_weight is not None and init_u8 is not None else ""
+        # ... then the token merging ratios (the hires one with the hires fix only), then Tiling
+        if tome != 0:
+            cond_weight += f", Token merging ratio: {tome}"
+        if tome_hr != 0 and init_u8 is None and payload.get("enable_hr"):
+            cond_weight += f", Token merging ratio hr: {tome_hr}"
         infotexts = [f"{prompt}\nNegative prompt: {negative}\nSteps: {steps}, Sampler: {sampler}, CFG scale: {cfg_scale}, "
                      f"Seed: {s}, Size: {width}x{height}" + cond_weight + (", Tiling: True" if tiling else "") for s in seeds]
         info = {"all_seeds": seeds, "all_subseeds": subseeds, "all_prompts": [prompt] * n,
@@ -334,6 +345,32 @@ class LocalGPUWorker(Worker):
             if opts.get("ESRGAN_tile_overlap") is not None:
                 out["upscaler_overlap"] = int(opts["ESRGAN_tile_overlap"])
         return out
+
+    @staticmethod
+    def _token_merging(payload: dict, img2img: bool):
+        """(first-pass ratio, hires ratio) of sdwui's token merging for the request, as processing.get_token_merging_ratio
+        resolves them; `opts.X` is override_settings["X"] if present, else the options of the sdwui this runs in, else 0.
+        A non-numeric value raises ValueError."""
+        overrides = payload.get("override_settings") or {}
+
+        def num(v):
+            if v is None:
+                return 0
+            if isinstance(v, bool) or not isinstance(v, (int, float, str)):
+                raise ValueError(f"token merging ratio {v!r} is not a number")
+            return float(v) if isinstance(v, str) else v   # float() raises ValueError for a non-numeric string
+
+        def opt(name):
+            if name in overrides:
+                return num(overrides[name])
+            import modules.shared
+            return num(getattr(getattr(modules.shared, "opts", None), name, None))
+
+        p_ratio, p_hr = num(payload.get("token_merging_ratio")), num(payload.get("token_merging_ratio_hr"))
+        o_ratio, o_hr, o_img = opt("token_merging_ratio"), opt("token_merging_ratio_hr"), opt("token_merging_ratio_img2img")
+        if img2img:
+            return p_ratio or ("token_merging_ratio" in overrides and o_ratio) or o_img or o_ratio, 0
+        return p_ratio or o_ratio, p_hr or o_hr or p_ratio or o_ratio
 
     @staticmethod
     def _tiling(payload: dict) -> bool:
