@@ -68,6 +68,14 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
     if (++spins > B200SD_SPIN_LIMIT) __trap();
   }
 }
+// Unbounded wait, for code after a setmaxnreg.inc whose budget is above the launch's register count: ptxas holds a
+// branch that contains a trap to the launch's count (128 registers at 512 threads) and spills the rest.  A warp-
+// specialised kernel uses it where the barrier is completed by TMA loads its producer issues after bounded waits of its
+// own, so a stuck ring still traps there.
+__device__ __forceinline__ void mbar_wait_unbounded(uint64_t* bar, uint32_t parity) {
+  while (!mbar_try_wait(bar, parity)) {
+  }
+}
 
 // ----------------------------------------------------------------------------------------------
 // TMA loads (tile mode). Coordinates innermost first. OOB elements are zero-filled.
