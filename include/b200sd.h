@@ -127,7 +127,8 @@ int b200sd_upsample2x(const void* X, long long pitch_x, void* Y, long long pitch
  * pad = pad_end = 0 on Y. */
 int b200sd_pad_circular(const void* X, long long pitch_x, void* Y, long long pitch_y, int NB, int H, int W, int C, int p,
                         int dtype, void* stream);
-/* row softmax of an fp16/bf16 matrix in place, fp32 math (VAE mid-block attention, d=512 single head). */
+/* row softmax of an fp16/bf16 matrix in place, fp32 math (VAE mid-block attention, d=512 single head).  Any cols >= 1
+ * (the VAE calls it with cols = latent pixels: 16384 at 1024^2, 36864 at 1536^2). */
 int b200sd_softmax_rows(void* S, long long lds, int rows, int cols, float scale, int dtype, void* stream);
 /* Y[rows, C] = silu(X) elementwise (emb_layers SiLU). */
 int b200sd_silu(const void* X, void* Y, long long n, int dtype, void* stream);

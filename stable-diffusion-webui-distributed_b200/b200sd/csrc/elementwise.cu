@@ -46,7 +46,7 @@ __global__ void upsample2x_kernel(const uint4* __restrict__ X, long long pitch_x
   }
 }
 
-// one CTA per row; in place; cols <= 16384
+// one CTA per row; in place; any cols >= 1 (three strided passes over the row: max, sum, normalise)
 template <bool kBf16>
 __global__ void softmax_rows_kernel(void* S, long long lds, int cols, float scale_log2) {
   pdl_trigger();

@@ -423,13 +423,18 @@ def test_layernorm(ops, rows, c):
 
 # ----------------------------------------------------------------------------------------------- small ops
 def test_upsample2x(ops):
+    for dt in (torch.float16, torch.bfloat16):
+        _upsample2x_case(ops, dt)
+
+
+def _upsample2x_case(ops, dt):
     g = _gen(31)
-    x = _rand((2, 8, 16, 64), g)
-    out = torch.empty((2, 16, 32, 64), device="cuda", dtype=torch.float16)
+    x = _rand((2, 8, 16, 64), g, dtype=dt)
+    out = torch.empty((2, 16, 32, 64), device="cuda", dtype=dt)
     ops.upsample2x(x, out)
     torch.cuda.synchronize()
     ref = x.repeat_interleave(2, dim=1).repeat_interleave(2, dim=2)
-    assert torch.equal(out, ref)
+    assert torch.equal(out, ref), dt
 
 
 def test_softmax_rows(ops):
@@ -442,24 +447,36 @@ def test_softmax_rows(ops):
 
 
 def test_silu_and_timestep_embedding(ops):
+    for dt in (torch.float16, torch.bfloat16):
+        _silu_and_timestep_embedding_case(ops, dt)
+
+
+def _silu_and_timestep_embedding_case(ops, dt):
     g = _gen(33)
-    x = _rand((20, 1280), g, 3.0)
+    x = _rand((20, 1280), g, 3.0, dtype=dt)
     out = torch.empty_like(x)
     ops.silu(x, out)
     t = torch.tensor([1.0, 51.0, 501.0, 951.0], device="cuda")
-    emb = torch.empty((4, 320), device="cuda", dtype=torch.float16)
+    emb = torch.empty((4, 320), device="cuda", dtype=dt)
     ops.timestep_embedding(t, emb)
     torch.cuda.synchronize()
-    assert_close("silu", out, F.silu(x.float()), atol=1e-3, rtol=2e-3)
+    # one rounding of the output: fp16 2^-11, bf16 2^-8 relative (the bf16 bounds are the fp16 ones scaled by 8 and 2)
+    k_silu, k_emb = (1, 1) if dt == torch.float16 else (8, 2)
+    assert_close(f"silu {dt}", out, F.silu(x.float()), atol=1e-3 * k_silu, rtol=2e-3 * k_silu)
     freqs = torch.exp(-math.log(10000.0) * torch.arange(160, device="cuda", dtype=torch.float32) / 160)
     args = t[:, None] * freqs[None]
     ref = torch.cat([torch.cos(args), torch.sin(args)], dim=-1)
-    assert_close("timestep_embedding", emb, ref, atol=2e-3, rtol=0)
+    assert_close(f"timestep_embedding {dt}", emb, ref, atol=2e-3 * k_emb, rtol=0)
 
 
 def test_fold_and_select_bias(ops):
+    for dt in (torch.float16, torch.bfloat16):
+        _fold_and_select_bias_case(ops, dt)
+
+
+def _fold_and_select_bias_case(ops, dt):
     g = _gen(34)
-    emb = _rand((20, 640), g)
+    emb = _rand((20, 640), g, dtype=dt)
     bias = torch.randn(640, generator=g, device="cuda")
     table = torch.empty((20, 640), device="cuda")
     ops.fold_bias(emb, bias, table)
@@ -467,23 +484,28 @@ def test_fold_and_select_bias(ops):
     cur = torch.empty(640, device="cuda")
     ops.select_step(table, step, cur)
     torch.cuda.synchronize()
-    assert torch.allclose(table, emb.float() + bias)
-    assert torch.equal(cur, table[7])
+    assert torch.allclose(table, emb.float() + bias), dt
+    assert torch.equal(cur, table[7]), dt
 
 
 def test_cfg_ddim_step_and_pack(ops):
+    for dt in (torch.float16, torch.bfloat16):
+        _cfg_ddim_step_and_pack_case(ops, dt)
+
+
+def _cfg_ddim_step_and_pack_case(ops, dt):
     g = _gen(35)
     b, hw = 3, 4096
     x = torch.randn((b, hw, 4), generator=g, device="cuda")
     x0 = x.clone()
-    xin = torch.zeros((2 * b, hw, 64), device="cuda", dtype=torch.float16)
+    xin = torch.zeros((2 * b, hw, 64), device="cuda", dtype=dt)
     ops.pack_unet_input(x, xin, 1.0)
-    eps = torch.zeros((2 * b, hw, 32), device="cuda", dtype=torch.float16)
-    eps[..., :4] = _rand((2 * b, hw, 4), g)
+    eps = torch.zeros((2 * b, hw, 32), device="cuda", dtype=dt)
+    eps[..., :4] = _rand((2 * b, hw, 4), g, dtype=dt)
     coef = torch.tensor([[0.3, 0.95, 0.4, 0.92], [0.5, 0.87, 0.6, 0.8]], device="cuda")
     step = torch.tensor([1], device="cuda", dtype=torch.int32)
     torch.cuda.synchronize()
-    assert torch.equal(xin[:b, :, :4], x0.half()) and torch.equal(xin[b:, :, :4], x0.half())
+    assert torch.equal(xin[:b, :, :4], x0.to(dt)) and torch.equal(xin[b:, :, :4], x0.to(dt))
     assert float(xin[..., 4:].abs().max()) == 0.0
     ops.cfg_ddim_step(eps, x, xin, 7.0, coef, step)
     torch.cuda.synchronize()
@@ -493,7 +515,7 @@ def test_cfg_ddim_step_and_pack(ops):
     ref = 0.6 * pred_x0 + 0.8 * e
     assert torch.allclose(x, ref, atol=1e-4, rtol=1e-5)
     assert int(step.item()) == 2
-    assert torch.equal(xin[b:, :, :4], x.half())
+    assert torch.equal(xin[:b, :, :4], x.to(dt)) and torch.equal(xin[b:, :, :4], x.to(dt))
 
 
 def test_cfg_euler_a_step(ops):
@@ -517,14 +539,19 @@ def test_cfg_euler_a_step(ops):
 
 
 def test_quantize_u8(ops):
+    for dt in (torch.float16, torch.bfloat16):
+        _quantize_u8_case(ops, dt)
+
+
+def _quantize_u8_case(ops, dt):
     g = _gen(37)
-    img = torch.zeros((2, 1000, 32), device="cuda", dtype=torch.float16)
-    img[..., :3] = _rand((2, 1000, 3), g, 0.8)
+    img = torch.zeros((2, 1000, 32), device="cuda", dtype=dt)
+    img[..., :3] = _rand((2, 1000, 3), g, 0.8, dtype=dt)
     out = torch.empty((2, 1000, 3), device="cuda", dtype=torch.uint8)
     ops.quantize_u8(img, out)
     torch.cuda.synchronize()
     ref = (255.0 * ((img[..., :3].float() + 1.0) * 0.5).clamp(0, 1)).to(torch.uint8)
-    assert torch.equal(out, ref)
+    assert torch.equal(out, ref), dt
 
 
 
