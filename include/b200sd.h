@@ -142,6 +142,14 @@ int b200sd_fold_bias(const void* emb, long long lde, const float* bias, float* t
                      void* stream);
 /* cur[0..n) = table[*step_counter][0..n) : selects this sampler step's rows on the device (graph replay safe). */
 int b200sd_select_step(const float* table, long long row_len, const int* step_counter, float* cur, void* stream);
+/* prompt editing: ctx[row][0..cap) = bank[e][0..entry_len[e]) followed by zeros, and kv_len[row] = entry_len[e], where
+ * e = sched[*step_counter][row].  bank [n_entries][cap][ctx_dim] and ctx [rows][cap][ctx_dim] are fp16 or bf16 (a
+ * 16-byte copy: the type does not enter), 16-byte aligned, ctx_dim % 8 == 0; sched [*][rows] int32 (the caller keeps
+ * its entries in [0, n_entries); out-of-range ones are clamped); entry lengths are clamped to [1, cap].  Reads the
+ * step counter on the device like b200sd_select_step (graph replay safe). */
+int b200sd_select_context(const void* bank, const int* entry_len, int n_entries, const int* sched,
+                          const int* step_counter, void* ctx, int* kv_len, int rows, int cap, int ctx_dim,
+                          void* stream);
 /* latents fp32 NHWC [B,HW,4] -> UNet input [2B,HW,pitch] (cond half and uncond half identical, channels >= 4
  * untouched: they are zero from allocation) */
 int b200sd_pack_unet_input(const float* x, void* xin, long long pitch, int B, int HW, float in_scale, int dtype,

@@ -114,6 +114,28 @@ __global__ void select_step_kernel(const float* __restrict__ table, long long ro
     cur[i] = src[i];
 }
 
+// ctx[row] = bank[sched[*step][row]] up to that entry's length, zero up to cap; kv_len[row] = the length.  One grid row
+// per context row, 16-byte vectors (the copy is bitwise for fp16 and bf16 alike).
+__global__ void select_context_kernel(const uint4* __restrict__ bank, const int* __restrict__ entry_len, int n_entries,
+                                      const int* __restrict__ sched, const int* step, uint4* __restrict__ ctx,
+                                      int* kv_len, int rows, int cap, int vec_per_token) {
+  pdl_trigger();
+  pdl_wait();
+  const int row = blockIdx.y;
+  int e = sched[static_cast<long long>(*step) * rows + row];
+  e = e < 0 ? 0 : (e >= n_entries ? n_entries - 1 : e);
+  int len = entry_len[e];
+  len = len < 1 ? 1 : (len > cap ? cap : len);
+  const long long per_row = static_cast<long long>(cap) * vec_per_token;
+  const long long valid = static_cast<long long>(len) * vec_per_token;
+  const uint4* src = bank + e * per_row;
+  uint4* dst = ctx + row * per_row;
+  for (long long i = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x; i < per_row;
+       i += static_cast<long long>(gridDim.x) * blockDim.x)
+    dst[i] = i < valid ? src[i] : make_uint4(0u, 0u, 0u, 0u);
+  if (blockIdx.x == 0 && threadIdx.x == 0) kv_len[row] = len;
+}
+
 // ---------------------------------------------------------------------------------------------
 // latents: x fp32 [B][HW][4]; UNet input xin [2B][HW][pitch] (channels 0..3 written, rest stay zero)
 template <bool kBf16>
@@ -476,6 +498,25 @@ extern "C" int b200sd_select_step(const float* table, long long row_len, const i
   long long blocks = (row_len + 255) / 256;
   if (blocks > kNumSms) blocks = kNumSms;
   launch_pdl(select_step_kernel, dim3(static_cast<int>(blocks)), dim3(256), 0, ST(stream), table, row_len, step_counter, cur);
+  RET_LAUNCH();
+}
+
+extern "C" int b200sd_select_context(const void* bank, const int* entry_len, int n_entries, const int* sched,
+                                     const int* step_counter, void* ctx, int* kv_len, int rows, int cap, int ctx_dim,
+                                     void* stream) {
+  if (rows < 1 || n_entries < 1 || cap < 1 || ctx_dim < 8 || ctx_dim % 8 || bank == nullptr || ctx == nullptr ||
+      entry_len == nullptr || sched == nullptr || step_counter == nullptr || kv_len == nullptr ||
+      ((reinterpret_cast<uintptr_t>(bank) | reinterpret_cast<uintptr_t>(ctx)) & 15))
+    return B200SD_ERR_INVALID;
+  const int vec_per_token = ctx_dim / 8;
+  const long long per_row = static_cast<long long>(cap) * vec_per_token;
+  long long bx = (per_row + 255) / 256;
+  const long long max_bx = (4LL * kNumSms + rows - 1) / rows;   // about four CTAs per SM over all rows
+  if (bx > max_bx) bx = max_bx;
+  if (rows > 65535) return B200SD_ERR_INVALID;
+  launch_pdl(select_context_kernel, dim3(static_cast<int>(bx), rows), dim3(256), 0, ST(stream),
+             reinterpret_cast<const uint4*>(bank), entry_len, n_entries, sched, step_counter,
+             reinterpret_cast<uint4*>(ctx), kv_len, rows, cap, vec_per_token);
   RET_LAUNCH();
 }
 

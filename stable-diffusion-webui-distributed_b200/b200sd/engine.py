@@ -16,6 +16,7 @@ from . import ops
 from . import samplers as S
 from .clip_text import CAPTURE_LOCK as _CAPTURE_LOCK, Cond, Conditioner
 from .config import UNET_PREFIX, CLIPConfig, UNetConfig, VAEConfig
+from .prompts import schedule_index
 from .unet_exec import MAX_CONTROLS, ControlNetWeights, TimeEmbedding, UNetProgram, UNetWeights
 from .vae_exec import VAEDecoderProgram, VAEDecoderWeights, VAEEncoderProgram, VAEEncoderWeights
 
@@ -182,6 +183,17 @@ SAMPLERS = {"DDIM": ("ddim", None), "Euler a": ("euler_a", "uniform"), "Euler": 
             "DPM++ 2M": ("dpmpp_2m", "karras"), "DPM++ 2M Karras": ("dpmpp_2m", "karras"), **S.GENERIC}
 
 
+# sdwui's samplers flagged second_order (sd_samplers_kdiffusion.samplers_k_diffusion): two model evaluations per step,
+# and SamplerData.total_steps counts both, so prompt schedules run over steps x 2
+SECOND_ORDER = ("Heun", "DPM2", "DPM2 a", "DPM++ 2S a", "DPM++ SDE", "DPM2 Karras", "DPM2 a Karras",
+                "DPM++ 2S a Karras", "DPM++ SDE Karras")
+
+
+def total_steps(sampler: str, steps: int) -> int:
+    """sdwui SamplerData.total_steps: the steps a prompt schedule of the request is built over"""
+    return steps * 2 if sampler in SECOND_ORDER else steps
+
+
 # API scheduler labels (sdwui >= 1.9 sd_schedulers.schedulers: label or name) -> kdiffusion_sigmas scheduler
 SCHEDULERS = {"Uniform": "uniform", "uniform": "uniform", "Karras": "karras", "karras": "karras",
               "Exponential": "exponential", "exponential": "exponential", "Polyexponential": "polyexponential",
@@ -259,6 +271,15 @@ class Program:
         return len(self.ts) if self.fused else (len(self.sp.stages) if self.sp is not None else None)
 
 
+@dataclass
+class PromptSchedule:
+    """one prompt's sdwui schedule (prompts.prompt_schedule) for a sampling pass: the entries' token ids, tokenized
+    together so that they have one chunk count, and the step each entry ends at"""
+    ends: List[int]                              # end_at_step per entry, increasing
+    tokens: torch.Tensor                         # [E, 77 * k]
+    multipliers: Optional[torch.Tensor] = None   # [E, 77 * k] emphasis weights (None: all 1)
+
+
 # ------------------------------------------------------------------------------------------------ plans
 class Plan:
     """Everything shape-dependent for (images per call b, latent h x w) on one device.  tiling: the UNet's and the VAE
@@ -287,6 +308,9 @@ class Plan:
             self.lat[name] = torch.zeros((b, h * w, 4), device=dev, dtype=torch.float32)
         self.coefL = torch.zeros((MAX_STEPS, S.COEF_LD), device=dev, dtype=torch.float32)
         self.noise = None            # [rows, b, h*w, 4] fp32, persistent: captured graphs bake its address
+        # prompt editing (SDEngine._switch): the request's encoded entries [E, cap, ctx], their lengths, the entry of
+        # every [cond | uncond] row per evaluation [MAX_STEPS, 2b], and the context the "ctx" graph selects into
+        self.bank = self.bank_len = self.sched = self.ctx_stage = None
         self.graphs: Dict[str, torch.cuda.CUDAGraph] = {}
         self.graph_launches: Dict[str, int] = {}
         self.stage_ids: Dict[tuple, int] = {}   # (lincomb structure, evaluated latent) of a generic stage -> graph-name id
@@ -304,6 +328,40 @@ class Plan:
                 del self.graphs[name]
                 self.graph_launches.pop(name, None)
         return self.noise
+
+    def set_bank(self, cond_bank: torch.Tensor, uncond_bank: torch.Tensor):
+        """encoded schedule entries [Ec, Lc, ctx] and [Eu, Lu, ctx] -> the bank (cond entries first).  The bank grows in
+        powers of two and follows the context capacity; reallocating drops the "ctx" graphs that captured it."""
+        (ec, lc, c), (eu, lu, _) = cond_bank.shape, uncond_bank.shape
+        self.ensure_context(max(lc, lu))
+        cap, e = self.ctx_cap, ec + eu
+        if self.bank is None or self.bank.shape[0] < e or self.bank.shape[1] != cap:
+            rows = 4
+            while rows < e:
+                rows *= 2
+            dev, dt = self.x.device, self.unet.dt
+            self.bank = torch.zeros((rows, cap, c), device=dev, dtype=dt)
+            self.bank_len = torch.ones((rows,), device=dev, dtype=torch.int32)
+            self.ctx_stage = torch.zeros((2 * self.b, cap, c), device=dev, dtype=dt)
+            for name in [n for n in self.graphs if n.startswith("ctx")]:
+                del self.graphs[name]
+                self.graph_launches.pop(name, None)
+        if self.sched is None:
+            self.sched = torch.zeros((MAX_STEPS, 2 * self.b), device=self.x.device, dtype=torch.int32)
+        self.bank[:ec, :lc].copy_(cond_bank)
+        self.bank[ec:e, :lu].copy_(uncond_bank)
+        self.bank_len[:e].copy_(torch.tensor([lc] * ec + [lu] * eu, dtype=torch.int32))
+
+    def set_sched(self, row0: int, entries):
+        """rows row0.. of the schedule table: (cond entry, uncond entry) per evaluation, bank indices"""
+        rows = [[c] * self.b + [u] * self.b for c, u in entries]
+        self.sched[row0:row0 + len(rows)].copy_(torch.tensor(rows, dtype=torch.int32))
+
+    def switch_context(self, slots):
+        """the switch: select this evaluation's entries (device step counter) into the staging context, then project
+        the K/V of every attn2 of the UNet and of the ControlNet segments in `slots`"""
+        ops.select_context(self.bank, self.bank_len, self.sched, self.step, self.ctx_stage, self.unet.kv_len)
+        self.unet.project_context(self.ctx_stage, [self.unet.segments[s] for s in slots])
 
     @property
     def ctx_cap(self) -> int:
@@ -444,6 +502,9 @@ class SDEngine:
         self.variation = (None, 0.0)   # (subseed, subseed_strength) of the request being served: sdwui variation seeds
         self._y = None                 # SDXL vector conditioning of the run in progress
         self._windows = []             # (guidance_start, guidance_end) of the run's ControlNet unit in each slot
+        self._entries = None           # prompt editing: (cond ends, uncond ends, cond entries) of the run in progress
+        self._ybank = None             # ... and the entries' SDXL vector conditionings (cond, uncond)
+        self._last_entry = None        # (cond, uncond) bank entries the K/V buffers hold
         self._cap_stream = None
         self.last_unet_evals = 0
         self.graph_replayed_launches = 0   # b200sd kernels launched through graph replays (bench.py gpu_launches)
@@ -520,6 +581,23 @@ class SDEngine:
         empty_neg = self.clip.xl and bool((neg_tokens[:, 1:] == neg_tokens[:, -1:]).all())
         return (self.encode_prompts(tokens, width, height, multipliers=multipliers),
                 self.encode_prompts(neg_tokens, width, height, zero_txt=empty_neg, multipliers=neg_multipliers))
+
+    def _pass_conds(self, tokens, neg_tokens, width: int, height: int, multipliers, neg_multipliers, schedule):
+        """(cond, uncond, run_program's schedule) of one sampling pass.  schedule = (cond PromptSchedule, uncond
+        PromptSchedule) or None (the tokens).  Schedules of one entry per side are encoded as that entry for every image
+        and run as an unscheduled pass; otherwise every entry is encoded once and the pass switches between them."""
+        if schedule is None:
+            return (*self._conds(tokens, neg_tokens, width, height, multipliers, neg_multipliers), None)
+        cs, us = schedule
+        if len(cs.ends) == 1 and len(us.ends) == 1:
+            b = tokens.shape[0]
+            rows = lambda t: None if t is None else t[:1].expand(b, -1)  # noqa: E731
+            return (*self._conds(rows(cs.tokens), rows(us.tokens), width, height, rows(cs.multipliers),
+                                 rows(us.multipliers)), None)
+        if len(cs.ends) > MAX_STEPS or len(us.ends) > MAX_STEPS:
+            raise ValueError("too many prompt schedule entries")
+        cond, uncond = self._conds(cs.tokens, us.tokens, width, height, cs.multipliers, us.multipliers)
+        return cond, uncond, (cs.ends, us.ends)
 
     def _graph(self, plan: Plan, name: str, fn):
         """Run fn eagerly once (per-device kernel attribute setup must not happen under capture), then capture."""
@@ -665,14 +743,17 @@ class SDEngine:
     @torch.no_grad()
     def run_program(self, cond: torch.Tensor, uncond: torch.Tensor, x_start: torch.Tensor, pr: "Program", cfg_scale: float,
                     noises: Optional[torch.Tensor] = None, inpaint=None, controls=None,
-                    tiling: bool = False, image_cond=None, token_merging_ratio: float = 0.0) -> torch.Tensor:
+                    tiling: bool = False, image_cond=None, token_merging_ratio: float = 0.0,
+                    schedule=None) -> torch.Tensor:
         """cond/uncond [b, 77 * k, ctx] on device (cond and uncond may have different k); x_start [b, 4, h, w] fp32 (host or device) = Program.start(...): the start
         latents in the sampler's own space; noises [pr.draws, b, 4, h, w]: the per-image N(0,1) draws after the first;
         inpaint = (clean init latents [b, 4, h, w], latent mask [h * w]).  controls: ControlNet units, see _set_controls
         (None: no ControlNet).  tiling: the UNet's convs pad circularly (its own plan).  image_cond = (masked-image
         latents fp32 [b, 4, h, w], pixel mask uint8 [f*h, f*w] or None for all ones): an inpainting model's extra UNet
         input channels, packed once before sampling (required for a 9-channel UNet, refused for a 4-channel one).
-        token_merging_ratio: sdwui's token merging (its own plan; see merged_tokens).  Returns the final latents fp32
+        token_merging_ratio: sdwui's token merging (its own plan; see merged_tokens).  schedule = (cond ends, uncond
+        ends): prompt editing — cond / uncond are then the encoded entries of the two schedules [E, 77 * k, ctx] and
+        every model evaluation attends to its own entries (sdwui reconstruct_cond_batch).  Returns the final latents fp32
         [b, h*w, 4] (NHWC, a view of plan state)."""
         b, _, h, w = x_start.shape
         if pr.draws and (noises is None or noises.shape[0] < pr.draws):
@@ -690,9 +771,18 @@ class SDEngine:
             if controls and cond.y is not None:
                 raise ValueError("ControlNet is not served for SDXL")
             self._windows = self._set_controls(plan, controls) if controls else []
-            plan.set_context(cond.ctx, uncond.ctx)
-            # SDXL: the vector conditioning of [cond | uncond] enters through the time-embedding table (per-sample rows)
-            self._y = None if cond.y is None else torch.cat([cond.y, uncond.y]).to(self.device)
+            if schedule is None:
+                self._entries = self._ybank = None
+                plan.set_context(cond.ctx, uncond.ctx)
+                # SDXL: the vector conditioning of [cond | uncond] enters through the time-embedding table (per-sample
+                # rows)
+                self._y = None if cond.y is None else torch.cat([cond.y, uncond.y]).to(self.device)
+            else:
+                self._entries = (list(schedule[0]), list(schedule[1]), cond.ctx.shape[0])
+                self._ybank = None if cond.y is None else (cond.y.to(self.device), uncond.y.to(self.device))
+                self._y = None
+                self._last_entry = None
+                plan.set_bank(cond.ctx, uncond.ctx)
             masked = inpaint is not None
             if masked:   # (clean init latents [b, 4, h, w], latent mask [h * w])
                 plan.init.copy_(inpaint[0].to(self.device, torch.float32).permute(0, 2, 3, 1).reshape(b, h * w, 4))
@@ -714,6 +804,53 @@ class SDEngine:
             if masked:   # processing.py sample(): samples * nmask + init_latent * mask
                 ops.blend_latent(plan.x, plan.init, plan.latmask)
             return plan.x
+
+    # ------------------------------------------------------------------------------------------ prompt editing
+    def _entry(self, i: int) -> tuple:
+        """(cond, uncond) bank entries of model evaluation i"""
+        cond_ends, uncond_ends, ec = self._entries
+        return (schedule_index([(e, None) for e in cond_ends], i),
+                ec + schedule_index([(e, None) for e in uncond_ends], i))
+
+    def _set_sched(self, plan: Plan, i0: int, n: int):
+        """schedule-table rows 0..n-1 <- the entries of evaluations i0..i0+n-1 (no-op without a schedule)"""
+        if self._entries is not None and n:
+            plan.set_sched(0, [self._entry(i0 + k) for k in range(n)])
+
+    def _emb_table(self, plan: Plan, ts: torch.Tensor, i0: int) -> torch.Tensor:
+        """time-embedding rows of evaluations i0..: SDXL under a schedule takes each evaluation's vector conditioning
+        from its entries, one table per distinct entry pair"""
+        if self._ybank is None:
+            return self.temb.table(ts, self._y)
+        yc, yu = self._ybank
+        ec = self._entries[2]
+        groups: Dict[tuple, List[int]] = {}
+        for k in range(ts.numel()):
+            groups.setdefault(self._entry(i0 + k), []).append(k)
+        out = torch.empty((ts.numel(), plan.table.shape[1]), device=self.device, dtype=torch.float32)
+        for (c, u), idx in groups.items():
+            y = torch.cat([yc[c:c + 1].expand(plan.b, -1), yu[u - ec:u - ec + 1].expand(plan.b, -1)])
+            out[torch.tensor(idx, device=self.device)] = self.temb.table(ts[idx], y)
+        return out
+
+    def _switch(self, plan: Plan, i: int):
+        """before model evaluation i: replay the "ctx" graph when its entries differ from the ones the K/V buffers hold.
+        The graph reads the device step counter, i.e. the schedule-table row _set_sched filled for evaluation i."""
+        if self._entries is None:
+            return
+        e = self._entry(i)
+        if e == self._last_entry:
+            return
+        self._last_entry = e
+        slots = tuple(range(len(self._windows)))
+        name = "ctx" + self._control_name(plan, slots)
+        fn = lambda: plan.switch_context(slots)  # noqa: E731
+        g = self._graph(plan, name, fn)
+        if g is not None:
+            g.replay()
+            self.graph_replayed_launches += plan.graph_launches[name]
+        else:
+            fn()
 
     def _upload_noises(self, plan: Plan, noises: torch.Tensor, mix=None):
         """draws [D, b, 4, h, w] (host) -> rows of the plan's persistent noise stack, mixed as the program says"""
@@ -746,7 +883,8 @@ class SDEngine:
         else:
             step_fn = lambda a=(): plan.step_dpmpp_2m(cfg_scale, a)  # noqa: E731
         ts = torch.tensor(pr.ts, dtype=torch.float32)
-        plan.table[:n_evals].copy_(self.temb.table(ts, self._y))
+        self._set_sched(plan, 0, n_evals)
+        plan.table[:n_evals].copy_(self._emb_table(plan, ts, 0))
         self._control_tables(plan, ts)
         (plan.coef8 if len(pr.rows[0]) == 8 else plan.coef)[:n_evals].copy_(torch.tensor(pr.rows, dtype=torch.float32))
         steps = {}   # active ControlNet slots -> (graph name, step function, graph); no units: () for every evaluation
@@ -759,6 +897,7 @@ class SDEngine:
                 gname = name + self._control_name(plan, active)
                 steps[active] = (gname, fn, self._graph(plan, gname, fn))
             gname, fn, g = steps[active]
+            self._switch(plan, i)
             if g is not None:
                 g.replay()
                 self.graph_replayed_launches += plan.graph_launches[gname]
@@ -774,7 +913,8 @@ class SDEngine:
             return
         self._upload_noises(plan, noises if noises is not None else torch.zeros((0, plan.b, 4, plan.h, plan.w)), sp.mix)
         ts = torch.tensor([st.t for st in stages], dtype=torch.float32)
-        plan.table[:len(stages)].copy_(self.temb.table(ts, self._y))
+        self._set_sched(plan, 0, len(stages))
+        plan.table[:len(stages)].copy_(self._emb_table(plan, ts, 0))
         self._control_tables(plan, ts)
         plan.coefL[:len(stages)].copy_(torch.tensor([st.row() for st in stages], dtype=torch.float32))
         step_of = S.stage_steps(stages)
@@ -783,6 +923,7 @@ class SDEngine:
                 break
             name, fn, g = self._stage_graph(plan, st, cfg_scale, masked, sp.timestep_sampler,
                                             self._active(i, step_of[-1] + 1))
+            self._switch(plan, self.last_unet_evals)
             if g is not None:
                 g.replay()
                 self.graph_replayed_launches += plan.graph_launches[name]
@@ -810,7 +951,8 @@ class SDEngine:
             t = min(t_end, s + pid.h)
             stages = S.dpm_adaptive_attempt(s, t, t_of)
             ts = torch.tensor([st.t for st in stages], dtype=torch.float32)
-            plan.table[:3].copy_(self.temb.table(ts, self._y))
+            self._set_sched(plan, self.last_unet_evals, 3)
+            plan.table[:3].copy_(self._emb_table(plan, ts, self.last_unet_evals))
             self._control_tables(plan, ts)
             plan.coefL[:3].copy_(torch.tensor([st.row() for st in stages], dtype=torch.float32))
             active = self._active(accepted, max(pr.steps, 1)) if self._windows else ()
@@ -818,6 +960,7 @@ class SDEngine:
             ops.pack_unet_input(plan.x, plan.unet.xin, S.c_in(math.exp(-s)))
             for st in stages:
                 name, fn, g = self._stage_graph(plan, st, cfg_scale, masked, False, active)
+                self._switch(plan, self.last_unet_evals)
                 if g is not None:
                     g.replay()
                     self.graph_replayed_launches += plan.graph_launches[name]
@@ -940,7 +1083,7 @@ class SDEngine:
                 inpainting_fill: int = 1, multipliers: Optional[torch.Tensor] = None,
                 neg_multipliers: Optional[torch.Tensor] = None, controls=None, tiling: bool = False,
                 image_mask: Optional[torch.Tensor] = None, inpainting_mask_weight: float = 1.0,
-                token_merging_ratio: float = 0.0) -> torch.Tensor:
+                token_merging_ratio: float = 0.0, schedule=None) -> torch.Tensor:
         """img2img: VAE-encode the init images (posterior mean), noise them to t_enc, run the remaining part of the
         sampler's schedule, decode.  init_u8 uint8 [b, H, W, 3].  Returns uint8 [b, H, W, 3] on device.
         `latmask` fp32 [h * w] (b200sd.inpaint.prepare_mask): inpainting — the region with latmask 0 is held to the init
@@ -959,9 +1102,13 @@ class SDEngine:
         processed pixel mask (inpaint.InpaintMask.fill_mask), required with `latmask`; without a mask it is all ones.
         Other models ignore both arguments.
         `token_merging_ratio`: sdwui's token merging (tomesd) in the UNet's full-resolution self-attention; <= 0 does not
-        merge."""
+        merge.
+        `schedule` = (cond PromptSchedule, uncond PromptSchedule): prompt editing / alternation (sdwui's prompt
+        schedules over the sampler's total steps); tokens / neg_tokens then give only the batch size.  None: the
+        tokens for every step."""
         b = tokens.shape[0]
-        cond, uncond = self._conds(tokens, neg_tokens, init_u8.shape[2], init_u8.shape[1], multipliers, neg_multipliers)
+        cond, uncond, sched = self._pass_conds(tokens, neg_tokens, init_u8.shape[2], init_u8.shape[1], multipliers,
+                                               neg_multipliers, schedule)
         init = self.encode(init_u8, tiling)
         _, _, h, w = init.shape
         image_cond = None
@@ -976,7 +1123,7 @@ class SDEngine:
                 init = init + per_image_noise(seed, b, (4, h, w), 1, *self.variation)[0].to(self.device) * nm
         lat = self._sample_from(init, cond, uncond, seed, denoising_strength, steps, cfg_scale, sampler, scheduler,
                                 inpaint=None if latmask is None else (init, latmask), controls=controls, tiling=tiling,
-                                image_cond=image_cond, token_merging_ratio=token_merging_ratio)
+                                image_cond=image_cond, token_merging_ratio=token_merging_ratio, schedule=sched)
         return self.decode(lat, h, w, tiling, token_merging_ratio)
 
     def _txt2img_cond(self, b: int, h: int, w: int, tiling: bool):
@@ -989,7 +1136,8 @@ class SDEngine:
 
     def _sample_from(self, init: torch.Tensor, cond, uncond, seed: int, denoising_strength: float, steps: int,
                      cfg_scale: float, sampler: str, scheduler: Optional[str], inpaint=None, controls=None,
-                     tiling: bool = False, image_cond=None, token_merging_ratio: float = 0.0) -> torch.Tensor:
+                     tiling: bool = False, image_cond=None, token_merging_ratio: float = 0.0,
+                     schedule=None) -> torch.Tensor:
         """the img2img half of a sampler (also the second pass of the hires fix): `init` [b, 4, h, w] latents on the device,
         fresh per-image noise from `seed`, start at the noise level of t_enc.
         DDIM / PLMS: sdwui sd_samplers_timesteps.sample_img2img; k-diffusion samplers: KDiffusionSampler.sample_img2img."""
@@ -998,7 +1146,7 @@ class SDEngine:
         nz = per_image_noise(seed, b, (4, h, w), 1 + pr.draws, *self.variation)
         return self.run_program(cond, uncond, pr.start(nz[0].to(self.device), init), pr, cfg_scale,
                                 noises=nz[1:] if pr.draws else None, inpaint=inpaint, controls=controls, tiling=tiling,
-                                image_cond=image_cond, token_merging_ratio=token_merging_ratio)
+                                image_cond=image_cond, token_merging_ratio=token_merging_ratio, schedule=schedule)
 
     @torch.no_grad()
     def txt2img_hires(self, tokens: torch.Tensor, neg_tokens: torch.Tensor, seed: int, steps: int = 20,
@@ -1008,7 +1156,7 @@ class SDEngine:
                       neg_multipliers: Optional[torch.Tensor] = None, upscaler: str = "Latent",
                       upscaler_tile: int = 192, upscaler_overlap: int = 8, tiling: bool = False,
                       inpainting_mask_weight: float = 1.0, token_merging_ratio: float = 0.0,
-                      token_merging_ratio_hr: float = 0.0) -> torch.Tensor:
+                      token_merging_ratio_hr: float = 0.0, schedule=None, hr_schedule=None) -> torch.Tensor:
         """txt2img with sdwui's hires fix (StableDiffusionProcessingTxt2Img.sample / sample_hr_pass): first pass at
         (height, width), the `upscaler` to hr_scale x, a fresh per-image noise of the large shape from the same seeds,
         then the same sampler's img2img half from t_enc with `hr_steps` (0 = `steps`) steps, decode at the large size.
@@ -1020,8 +1168,14 @@ class SDEngine:
         pass the upscaled images' under an all-ones mask, s * (1 - inpainting_mask_weight).  sdwui conditions a "Latent"
         second pass with a weight below 1 on the float decode of the upscaled latents: refused.
         Token merging: the first pass (and its decode) at `token_merging_ratio`, the second at `token_merging_ratio_hr`.
+        `schedule` as for img2img, for the first pass; `hr_schedule` the second pass's own (sdwui hr_prompt /
+        hr_negative_prompt over the hires steps, with the first pass's steps as the base of its offsets), required with
+        `schedule`; without both the second pass takes the first pass's prompts.
         Returns uint8 [b, H*hr, W*hr, 3] on device."""
         from . import upscale
+        if schedule is not None and hr_schedule is None:
+            raise ValueError("a scheduled first pass needs the second pass's own schedule (hr_schedule): sdwui builds it "
+                             "over the hires steps")
         kind, _ = upscale.kind(upscaler)
         if self.inpainting and kind == "latent" and inpainting_mask_weight < 1:
             raise ValueError(f"hires upscaler {upscaler!r} with inpainting_mask_weight {inpainting_mask_weight} < 1 is not "
@@ -1031,10 +1185,10 @@ class SDEngine:
         h2, w2 = int(height * hr_scale) // 8, int(width * hr_scale) // 8
         if kind != "latent" and (int(height * hr_scale) % 8 or int(width * hr_scale) % 8):
             raise ValueError(f"hires upscaler {upscaler!r}: the target size must be a multiple of 8")
-        cond, uncond = self._conds(tokens, neg_tokens, width, height, multipliers, neg_multipliers)
+        cond, uncond, sched = self._pass_conds(tokens, neg_tokens, width, height, multipliers, neg_multipliers, schedule)
         lat = self._sample_txt(cond, uncond, seed, b, h, w, steps, cfg_scale, sampler, scheduler, tiling=tiling,
                                image_cond=self._txt2img_cond(b, h, w, tiling) if self.inpainting else None,
-                               token_merging_ratio=token_merging_ratio)
+                               token_merging_ratio=token_merging_ratio, schedule=sched)
         image_cond = None
         if kind == "latent":
             with self._ctx():
@@ -1054,35 +1208,40 @@ class SDEngine:
             init = self.encode(images.contiguous(), tiling)
             if self.inpainting:
                 image_cond = (self.encode_conditioning(images.contiguous(), None, inpainting_mask_weight, tiling), None)
-        if self.clip.xl:   # SDXL's vector conditioning carries the target size: the second pass gets its own (sdwui hr_c / hr_uc)
-            cond, uncond = self._conds(tokens, neg_tokens, w2 * 8, h2 * 8, multipliers, neg_multipliers)
+        if hr_schedule is not None:
+            cond, uncond, sched = self._pass_conds(tokens, neg_tokens, w2 * 8, h2 * 8, None, None, hr_schedule)
+        elif self.clip.xl:   # SDXL's vector conditioning carries the target size: the second pass gets its own (sdwui hr_c / hr_uc)
+            cond, uncond, sched = self._pass_conds(tokens, neg_tokens, w2 * 8, h2 * 8, multipliers, neg_multipliers,
+                                                   schedule)
         lat2 = self._sample_from(init, cond, uncond, seed, denoising_strength, hr_steps or steps, cfg_scale, sampler, scheduler,
-                                 tiling=tiling, image_cond=image_cond, token_merging_ratio=token_merging_ratio_hr)
+                                 tiling=tiling, image_cond=image_cond, token_merging_ratio=token_merging_ratio_hr,
+                                 schedule=sched)
         return self.decode(lat2, h2, w2, tiling, token_merging_ratio_hr)
 
     def _sample_txt(self, cond, uncond, seed: int, b: int, h: int, w: int, steps: int, cfg_scale: float, sampler: str,
                     scheduler: Optional[str], controls=None, tiling: bool = False, image_cond=None,
-                    token_merging_ratio: float = 0.0) -> torch.Tensor:
+                    token_merging_ratio: float = 0.0, schedule=None) -> torch.Tensor:
         pr = self.program(sampler, scheduler, steps)
         nz = per_image_noise(seed, b, (4, h, w), 1 + pr.draws, *self.variation)
         return self.run_program(cond, uncond, pr.start(nz[0]), pr, cfg_scale, noises=nz[1:] if pr.draws else None,
                                 controls=controls, tiling=tiling, image_cond=image_cond,
-                                token_merging_ratio=token_merging_ratio)
+                                token_merging_ratio=token_merging_ratio, schedule=schedule)
 
     @torch.no_grad()
     def txt2img(self, tokens: torch.Tensor, neg_tokens: torch.Tensor, seed: int, steps: int = 20, cfg_scale: float = 7.0,
                 height: int = 512, width: int = 512, sampler: str = "DDIM", scheduler: Optional[str] = None,
                 multipliers: Optional[torch.Tensor] = None, neg_multipliers: Optional[torch.Tensor] = None,
                 controls=None, tiling: bool = False, inpainting_mask_weight: float = 1.0,
-                token_merging_ratio: float = 0.0) -> torch.Tensor:
+                token_merging_ratio: float = 0.0, schedule=None) -> torch.Tensor:
         """Whole request for this engine's share: returns uint8 [b, H, W, 3] on device.  tokens [b, 77 * k] and
         neg_tokens [b, 77 * k'] with their optional emphasis multipliers of the same shapes (factory.tokenize_prompts).
         `controls`: ControlNet units as for img2img (None: none); `tiling` as for img2img.  An inpainting model gets
         sdwui's txt2img conditioning, which inpainting_mask_weight does not enter (it is taken for a uniform call).
-        `token_merging_ratio` as for img2img."""
+        `token_merging_ratio` and `schedule` as for img2img."""
         b = tokens.shape[0]
         h, w = height // 8, width // 8
-        cond, uncond = self._conds(tokens, neg_tokens, width, height, multipliers, neg_multipliers)
+        cond, uncond, sched = self._pass_conds(tokens, neg_tokens, width, height, multipliers, neg_multipliers, schedule)
         lat = self._sample_txt(cond, uncond, seed, b, h, w, steps, cfg_scale, sampler, scheduler, controls, tiling,
-                               self._txt2img_cond(b, h, w, tiling) if self.inpainting else None, token_merging_ratio)
+                               self._txt2img_cond(b, h, w, tiling) if self.inpainting else None, token_merging_ratio,
+                               sched)
         return self.decode(lat, h, w, tiling, token_merging_ratio)

@@ -266,6 +266,24 @@ def select_step(table: torch.Tensor, step_counter: torch.Tensor, cur: torch.Tens
     return cur
 
 
+def select_context(bank: torch.Tensor, entry_len: torch.Tensor, sched: torch.Tensor, step_counter: torch.Tensor,
+                   ctx: torch.Tensor, kv_len: torch.Tensor):
+    """ctx[row] = bank[sched[*step_counter, row]] zero-padded to the capacity, kv_len[row] = that entry's length.
+    bank [E, cap, ctx_dim] and ctx [rows, cap, ctx_dim] fp16/bf16; entry_len [E], sched [steps, rows], kv_len [rows]
+    int32"""
+    e, cap, c = bank.shape
+    rows = ctx.shape[0]
+    assert tuple(ctx.shape) == (rows, cap, c) and ctx.dtype == bank.dtype and bank.is_contiguous() and ctx.is_contiguous()
+    assert sched.dim() == 2 and sched.shape[1] == rows and sched.is_contiguous() and entry_len.numel() >= e
+    assert all(t.dtype == torch.int32 for t in (entry_len, sched, step_counter, kv_len)) and kv_len.numel() == rows
+    _dt(ctx)
+    rc = _lib.lib().b200sd_select_context(_p(bank), _p(entry_len), e, _p(sched), _p(step_counter), _p(ctx), _p(kv_len),
+                                          rows, cap, c, _stream())
+    check(rc, "b200sd_select_context")
+    _count()
+    return ctx
+
+
 def pack_unet_input(x: torch.Tensor, xin: torch.Tensor, in_scale: float = 1.0):
     """x fp32 [B, HW, 4]; xin [2B, HW, pitch]"""
     b, hw, _ = x.shape

@@ -9,8 +9,15 @@ What a remote sdwui does with `prompt` / `negative_prompt` before its text encod
     each framed as [BOS] + tokens + [EOS] padding + [EOS], with one multiplier per token.  A tower whose pad id is not EOS
     (SD 2.x's OpenCLIP: 0) gets that id after the first EOS of every chunk (process_tokens).
 
-Not interpreted (as text they reach the tokenizer unchanged): prompt editing `[a:b:when]`, alternation `[a|b]`,
-composable `AND`, textual-inversion embeddings and extra-network tags.
+Prompt editing `[from:to:when]` and alternation `[a|b]` (prompt_parser.get_learned_conditioning_prompt_schedules):
+prompt_schedule turns a prompt into [(end_at_step, text)]; the engine encodes each text once and switches the
+cross-attention context per model evaluation (schedule_index: sdwui's reconstruct_cond_batch).  Known parity gap: sdwui
+parses with lark's Earley parser, which resolves the ambiguity between a group and a run of two or more stray bracket or
+colon characters right after its closer in a way that depends on the rest of the prompt (`x [b:c:4]]] y` and
+`[a:b:5]):` stay literal text there, `[a:1]:` does not); prompt_schedule always parses such a group.
+
+Not interpreted (as text they reach the tokenizer unchanged): composable `AND`, textual-inversion embeddings and
+extra-network tags.
 """
 import re
 from typing import Callable, List, Optional, Sequence, Tuple
@@ -127,3 +134,167 @@ def tokenize_prompt(text: str, tokenize: Callable[[str], List[int]], bos: int, e
     segs = [((), w, True) if (t == "BREAK" and w == -1) else (tokenize(t), w, False)
             for t, w in parse_prompt_attention(text)]
     return chunk_tokens(segs, bos, eos, comma, pad=pad)
+
+
+# ------------------------------------------------------------------------------------------------ prompt editing
+# sdwui's schedule grammar (prompt_parser.schedule_parser):
+#   start: (prompt | stray "[", "]", "(", ")", ":")*     prompt: (emphasized | scheduled | alternate | plain | space)*
+#   emphasized: "(" prompt ")" | "(" prompt ":" prompt ")" | "[" prompt "]"
+#   scheduled: "[" [prompt ":"] prompt ":" [space] NUMBER [space] "]"      alternate: "[" prompt ("|" [prompt])+ "]"
+# A prompt holds no stray bracket, colon or bar, so every group is closed by the nearest matching closer; an opener
+# whose group is not one of the forms above is a stray character of the top level.  A bar outside an alternation, or a
+# backslash that escapes nothing, makes the prompt unparseable: it is then used as it is for every step.
+_NUMBER = re.compile(r"\s*([+-]?(?:[0-9]+(?:\.[0-9]*)?|\.[0-9]+)(?:[eE][+-]?[0-9]+)?)\s*")
+_PLAIN = re.compile(r"[^\\\[\]():|]+")
+
+
+class _Unparsable(Exception):
+    pass
+
+
+def _escape(s: str, j: int) -> str:
+    if j + 1 >= len(s) or s[j + 1] == "\n":
+        raise _Unparsable
+    return s[j:j + 2]
+
+
+def _group(s: str, i: int):
+    """s[i] is "[" or "(": (nodes of the group, index after its closer), or None if s[i] opens none of the grammar's
+    forms.  Nodes: text, ("edit", before nodes or None, after nodes, number text), ("alt", [nodes per option])."""
+    close = "]" if s[i] == "[" else ")"
+    segs: List[list] = [[]]
+    seps: List[str] = []
+    j = i + 1
+    while j < len(s):
+        c = s[j]
+        if c == "\\":
+            segs[-1].append(_escape(s, j))
+            j += 2
+        elif c in "[(":
+            r = _group(s, j)
+            if r is None:
+                return None
+            segs[-1].extend(r[0])
+            j = r[1]
+        elif c == close:
+            break
+        elif c in ")]":
+            return None
+        elif c in ":|":
+            seps.append(c)
+            segs.append([])
+            j += 1
+        else:
+            m = _PLAIN.match(s, j)
+            segs[-1].append(m.group(0))
+            j = m.end()
+    else:
+        return None
+    end = j + 1
+    if not seps or (close == ")" and seps == [":"]):   # emphasis: the brackets stay text for parse_prompt_attention
+        out = [s[i]]
+        for k, seg in enumerate(segs):
+            out += ([":"] if k else []) + seg
+        return out + [close], end
+    if close == ")":
+        return None
+    if all(c == "|" for c in seps):
+        return [("alt", segs)], end
+    if all(c == ":" for c in seps) and len(seps) <= 2 and all(isinstance(t, str) for t in segs[-1]):
+        m = _NUMBER.fullmatch("".join(segs[-1]))
+        if m:
+            return [("edit", segs[0] if len(seps) == 2 else None, segs[-2], m.group(1))], end
+    return None
+
+
+def _parse_schedule(s: str) -> list:
+    nodes: list = []
+    j = 0
+    while j < len(s):
+        c = s[j]
+        if c == "\\":
+            nodes.append(_escape(s, j))
+            j += 2
+        elif c == "|":
+            raise _Unparsable
+        elif c in "[(" and (r := _group(s, j)) is not None:
+            nodes.extend(r[0])
+            j = r[1]
+        elif c in "[]():":
+            nodes.append(c)
+            j += 1
+        else:
+            m = _PLAIN.match(s, j)
+            nodes.append(m.group(0))
+            j = m.end()
+    return nodes
+
+
+def prompt_schedule(text: str, steps: int, hires_steps: Optional[int] = None,
+                    use_old_scheduling: bool = False) -> List[Tuple[int, str]]:
+    """sdwui prompt_parser.get_learned_conditioning_prompt_schedules for one prompt: [(end_at_step, text)] in step
+    order, the last entry ending at the run's steps.  `[from:to:when]` is `from` up to step `when` and `to` after it
+    (`[to:when]`: nothing, then `to`); `[a|b|...]` takes option (step - 1) % n at every step.  `when` with a "." is a
+    fraction of the steps, without one an absolute step; for the hires pass (hires_steps: its steps, `steps`: the
+    first pass's) a fraction counts from 1.0 and a step from `steps`.  use_old_scheduling: `when` < 1 is a fraction,
+    anything else a step, and no hires offsets."""
+    try:
+        nodes = _parse_schedule(text)
+    except _Unparsable:
+        return [(hires_steps if hires_steps is not None and not use_old_scheduling else steps, text)]
+    if hires_steps is None or use_old_scheduling:
+        int_offset, flt_offset = 0, 0.0
+    else:
+        int_offset, flt_offset, steps = steps, 1.0, hires_steps
+    bounds = {steps}
+
+    def when(num: str) -> int:
+        v = float(num)
+        if use_old_scheduling:
+            v = v * steps if v < 1 else v
+        elif "." in num:
+            v = (v - flt_offset) * steps
+        else:
+            v = v - int_offset
+        return steps if v >= steps else int(v)
+
+    def resolve(ns):   # number text -> clamped step; collects the boundaries
+        out = []
+        for n in ns:
+            if isinstance(n, str):
+                out.append(n)
+            elif n[0] == "edit":
+                w = when(n[3])
+                if w >= 1:
+                    bounds.add(w)
+                out.append(("edit", None if n[1] is None else resolve(n[1]), resolve(n[2]), w))
+            else:
+                bounds.update(range(1, steps + 1))
+                out.append(("alt", [resolve(o) for o in n[1]]))
+        return out
+
+    def render(ns, step: int) -> str:
+        parts = []
+        for n in ns:
+            if isinstance(n, str):
+                parts.append(n)
+            elif n[0] == "edit":
+                if step <= n[3]:
+                    parts.append("" if n[1] is None else render(n[1], step))
+                else:
+                    parts.append(render(n[2], step))
+            else:
+                parts.append(render(n[1][(step - 1) % len(n[1])], step))
+        return "".join(parts)
+
+    tree = resolve(nodes)
+    return [(t, render(tree, t)) for t in sorted(bounds)]
+
+
+def schedule_index(schedule: Sequence[Tuple[int, str]], step: int) -> int:
+    """the entry model evaluation `step` (from 0) uses: the first whose end_at_step >= step, entry 0 if none
+    (sdwui prompt_parser.reconstruct_cond_batch)"""
+    for i, (end, _) in enumerate(schedule):
+        if step <= end:
+            return i
+    return 0

@@ -296,13 +296,17 @@ class UNetProgram:
             assert all(v == self.ctx_len for v in lengths), "a context shorter than the capacity needs grow_context"
         if l < self.ctx_len:   # zero rows up to the capacity: their keys are masked, their values finite
             ctx = torch.cat([ctx, ctx.new_zeros((n, self.ctx_len - l, c))], dim=1)
-        l = self.ctx_len
-        ctx2 = ctx.reshape(n * l, c)
-        for w, ctx_kv in [(self.w, self.ctx_kv)] + [(s.w, s.ctx_kv) for s in self.segments if s is not None]:
-            for key, buf in ctx_kv.items():
-                ops.linear(ctx2, w.t[key + ".attn2.kv.w"], buf.reshape(n * l, -1), bias=w.t[key + ".attn2.kv.b"])
+        self.project_context(ctx, [s for s in self.segments if s is not None])
         if self.ctx_len != self.ctx_len0:
             self.kv_len.copy_(torch.tensor(lengths, dtype=torch.int32))
+
+    def project_context(self, ctx: torch.Tensor, segments):
+        """K/V of every attn2 of the UNet and of the ControlNet `segments` from ctx [N, ctx_len, context_dim]"""
+        n, l = self.n, self.ctx_len
+        ctx2 = ctx.reshape(n * l, ctx.shape[-1])
+        for w, ctx_kv in [(self.w, self.ctx_kv)] + [(s.w, s.ctx_kv) for s in segments]:
+            for key, buf in ctx_kv.items():
+                ops.linear(ctx2, w.t[key + ".attn2.kv.w"], buf.reshape(n * l, -1), bias=w.t[key + ".attn2.kv.b"])
 
     def grow_context(self, cap: int):
         """Reallocate every cross-attention K/V buffer with `cap` rows per image (cap > ctx_len) and point the program's

@@ -221,14 +221,36 @@ class LocalGPUWorker(Worker):
         vocab = eng.clip_cfg.vocab
         pad = getattr(eng.clip_cfg, "pad_id", None)   # the token after each chunk's first EOS (SD 2.x: 0)
         mult_all = None
+        # prompt editing / alternation: sdwui's schedules over the sampler's total steps.  A prompt whose schedule has
+        # one entry is that entry's text (the prompt itself without schedule syntax) for every step.
+        sched_kw, hr_kw = {}, {}
+        cond_text, neg_text = prompt, negative
+        if "prompt_tokens" not in payload:
+            from b200sd.engine import total_steps
+            old = self._use_old_scheduling(payload)
+            base = total_steps(sampler, steps)
+            cs = self._schedule(prompt, base, None, old, vocab, pad)
+            us = self._schedule(negative, base, None, old, vocab, pad)
+            if len(cs[0].ends) > 1 or len(us[0].ends) > 1:
+                sched_kw["schedule"] = (cs[0], us[0])
+            cond_text, neg_text = cs[1][0], us[1][0]
+            if payload.get("enable_hr") and not payload.get("init_images"):
+                # sdwui calculate_hr_conds: hr_prompt / hr_negative_prompt (empty: the first pass's), over the hires
+                # steps with the first pass's as the base of the offsets
+                hires = total_steps(sampler, int(payload.get("hr_second_pass_steps") or 0) or steps)
+                hc = self._schedule(payload.get("hr_prompt") or prompt, base, hires, old, vocab, pad)
+                hu = self._schedule(payload.get("hr_negative_prompt") or negative, base, hires, old, vocab, pad)
+                if sched_kw or len(hc[1]) > 1 or len(hu[1]) > 1 or (hc[1][0], hu[1][0]) != (cond_text, neg_text):
+                    hr_kw["hr_schedule"] = (hc[0], hu[0])
         if "prompt_tokens" in payload:  # benchmark / tests hand pre-tokenised prompts through
             tok_all = torch.as_tensor(payload["prompt_tokens"]).long().reshape(-1, 77)
         else:   # sdwui prompt syntax: emphasis weights, BREAK, 77-token chunks
-            tok_all, mult_all = tokenize_prompts([prompt] * batch, vocab, pad)
-        neg_all, neg_mult = tokenize_prompts([negative] * batch, vocab, pad)
+            tok_all, mult_all = tokenize_prompts([cond_text] * batch, vocab, pad)
+        neg_all, neg_mult = tokenize_prompts([neg_text] * batch, vocab, pad)
         # emphasis multipliers reach the engine only when some weight differs from 1 (all 1 is the unweighted path)
         weighted = lambda m: m is not None and bool((m != 1.0).any())  # noqa: E731
         weights = {"neg_multipliers": neg_mult} if weighted(neg_mult) else {}
+        weights.update(sched_kw)
         if controls:   # a payload without ControlNet units reaches the engine with exactly the arguments it always had
             weights["controls"] = controls
         tiling = self._tiling(payload)
@@ -260,7 +282,7 @@ class LocalGPUWorker(Worker):
                 hr_scale = float(payload.get("hr_scale") or 2.0)
                 if payload.get("hr_resize_x") and payload.get("hr_resize_y"):
                     hr_scale = float(payload["hr_resize_x"]) / width
-                hires = dict(weights, **tome_kw)
+                hires = dict(weights, **tome_kw, **hr_kw)
                 if tome_hr > 0:
                     hires["token_merging_ratio_hr"] = float(tome_hr)
                 hires.update(self._hires_upscaler(payload, width, height, hr_scale))
@@ -371,6 +393,27 @@ class LocalGPUWorker(Worker):
         if img2img:
             return p_ratio or ("token_merging_ratio" in overrides and o_ratio) or o_img or o_ratio, 0
         return p_ratio or o_ratio, p_hr or o_hr or p_ratio or o_ratio
+
+    @staticmethod
+    def _schedule(text: str, steps: int, hires_steps, old: bool, vocab: int, pad):
+        """(PromptSchedule of a prompt, its entries' texts): sdwui's schedule, every entry tokenized in one call so
+        that all have the chunk count of the longest"""
+        from b200sd.engine import PromptSchedule
+        from b200sd.factory import tokenize_prompts
+        from b200sd.prompts import prompt_schedule
+        sch = prompt_schedule(text, steps, hires_steps, old)
+        ids, mult = tokenize_prompts([t for _, t in sch], vocab, pad)
+        return PromptSchedule([e for e, _ in sch], ids, mult if bool((mult != 1.0).any()) else None), [t for _, t in sch]
+
+    @staticmethod
+    def _use_old_scheduling(payload: dict) -> bool:
+        """sdwui's use_old_scheduling option: the request's override_settings, then the options of the sdwui this runs
+        in, then False"""
+        value = (payload.get("override_settings") or {}).get("use_old_scheduling")
+        if value is None:
+            import modules.shared
+            value = getattr(getattr(modules.shared, "opts", None), "use_old_scheduling", False)
+        return bool(value)
 
     @staticmethod
     def _tiling(payload: dict) -> bool:
