@@ -290,6 +290,24 @@ int b200sd_tome_merge(const void* X, long long pitch_x, const int* members, cons
 int b200sd_tome_unmerge_add(const void* R, long long pitch_r, const void* Y, long long pitch_y, const int* slot,
                             void* out, long long pitch_o, int B, int N, int Nm, int C, int dtype, void* stream);
 
+/* ---- LoRA networks merged into packed weights (sdwui networks.py network_apply_weights, `<lora:name:te:unet>`) ---- */
+/* One target: W[rows, cols] (row pitch ldw elements, fp16 / bf16) is rewritten from its pristine copy P (same layout and
+ * pitch) as W[i,k] = round_rn(P[i,k] + s), s = sum_{j < R} U[i,j] * D[j,k] accumulated in fp32 by fmaf in ascending j
+ * from 0 (bitwise the same on every device and run, whatever the tiling); where s == 0 (R == 0: a restore; a zero row of
+ * U) W = P bitwise.  U [rows, R] and D [R, cols] are fp32, row-major and dense.  W must not overlap P, U or D. */
+typedef struct b200sd_lora_target {
+  void* W;
+  const void* P;
+  const float* U;
+  const float* D;
+  long long ldw;
+  int rows, cols, R;
+  int reserved; /* 0 */
+} b200sd_lora_target;
+/* every target of the DEVICE-resident table targets[n_targets] in one persistent launch (register-tiled fp32 FMA; the
+ * rank loops in chunks of 32).  Targets must not overlap each other's W. */
+int b200sd_lora_merge(const b200sd_lora_target* targets, int n_targets, int dtype, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

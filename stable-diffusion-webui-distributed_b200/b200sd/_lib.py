@@ -22,6 +22,21 @@ class Epilogue(ctypes.Structure):
     ]
 
 
+class LoraTarget(ctypes.Structure):
+    """struct b200sd_lora_target"""
+    _fields_ = [
+        ("W", ctypes.c_void_p),
+        ("P", ctypes.c_void_p),
+        ("U", ctypes.c_void_p),
+        ("D", ctypes.c_void_p),
+        ("ldw", ctypes.c_longlong),
+        ("rows", ctypes.c_int),
+        ("cols", ctypes.c_int),
+        ("R", ctypes.c_int),
+        ("reserved", ctypes.c_int),
+    ]
+
+
 EPI_GEGLU = 1
 EPI_SILU = 2
 EPI_LRELU = 4

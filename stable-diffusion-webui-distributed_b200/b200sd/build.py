@@ -10,7 +10,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libb200sd.so")
 SOURCES = ["api.cu", "gemm_conv_tc.cu", "attention_tc.cu", "host_util.cu", "norm_kernels.cu", "elementwise.cu",
-           "upscale_kernels.cu", "pad_kernels.cu", "inpaint_kernels.cu", "tome_kernels.cu"]
+           "upscale_kernels.cu", "pad_kernels.cu", "inpaint_kernels.cu", "tome_kernels.cu", "lora_kernels.cu"]
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
     "-Xcompiler", "-fPIC", "--expt-relaxed-constexpr",

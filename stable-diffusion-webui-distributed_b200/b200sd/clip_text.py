@@ -21,6 +21,7 @@ import torch
 import torch.nn.functional as F
 
 from .config import CLIP_PREFIX, OPENCLIP_PREFIX, XL_PREFIX0, XL_PREFIX1, CLIPConfig
+from .weights import Placement
 
 
 CAPTURE_LOCK = threading.Lock()   # CUDA graph captures are serialised across the per-device worker threads (engine.py too)
@@ -42,6 +43,13 @@ def emphasis(z: torch.Tensor, mult: torch.Tensor) -> torch.Tensor:
     return zf.to(z.dtype)
 
 
+def _placements(w: Dict[str, torch.Tensor], prefix: str) -> Dict[str, Placement]:
+    """ldm key -> Placement of every linear weight of a tower's `w` (stored as in the checkpoint: identity placements;
+    OpenCLIP's attn.in_proj_weight holds q, k and v as its three row blocks)"""
+    return {prefix + k: Placement(k, tuple(v.shape)) for k, v in w.items()
+            if (k.endswith(".weight") and v.dim() == 2 and "embedding" not in k) or k.endswith(".in_proj_weight")}
+
+
 def _attend(q, k, v, mask):
     d = q.shape[-1]
     return torch.softmax((q @ k.transpose(-1, -2)).float() * d ** -0.5 + mask, dim=-1).to(q.dtype) @ v
@@ -51,7 +59,9 @@ class ClipText:
     def __init__(self, sd: Dict[str, torch.Tensor], cfg: CLIPConfig, device, dtype=torch.float16, prefix: str = CLIP_PREFIX):
         self.cfg, self.device, self.dtype = cfg, device, dtype
         n = len(prefix)
+        self.prefix = prefix
         self.w = {k[n:]: v.to(device=device, dtype=dtype) for k, v in sd.items() if k.startswith(prefix)}
+        self.place = _placements(self.w, prefix)
 
     @torch.no_grad()
     def hidden(self, tokens: torch.Tensor, layers: int) -> torch.Tensor:
@@ -92,7 +102,9 @@ class OpenClipText:
         self.width, self.layers, self.heads = ((cfg.xl_width, cfg.xl_layers, cfg.xl_heads) if cfg.xl_width else
                                                (cfg.width, cfg.layers, cfg.heads))
         n = len(prefix)
+        self.prefix = prefix
         self.w = {k[n:]: v.to(device=device, dtype=dtype) for k, v in sd.items() if k.startswith(prefix)}
+        self.place = _placements(self.w, prefix)
 
     def _blocks(self, x: torch.Tensor, start: int, stop: int, mask: torch.Tensor) -> torch.Tensor:
         """resblocks [start, stop) on the residual stream x [B, n, W]"""

@@ -52,4 +52,4 @@ int make_tmap_sw64(CUtensorMap* out, const void* base, int rank, const uint64_t*
 
 }  // namespace b200sd
 
-extern "C" const char* b200sd_version(void) { return "b200sd 0.12 sm_90a"; }
+extern "C" const char* b200sd_version(void) { return "b200sd 0.13 sm_90a"; }

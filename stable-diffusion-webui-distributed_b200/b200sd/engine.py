@@ -12,6 +12,7 @@ from typing import Dict, List, Optional, Tuple
 
 import torch
 
+from . import lora as L
 from . import ops
 from . import samplers as S
 from .clip_text import CAPTURE_LOCK as _CAPTURE_LOCK, Cond, Conditioner
@@ -508,6 +509,10 @@ class SDEngine:
         self._cap_stream = None
         self.last_unet_evals = 0
         self.graph_replayed_launches = 0   # b200sd kernels launched through graph replays (bench.py gpu_launches)
+        self._lora_set = ()            # identity of the LoRA networks merged into the weights; () = pristine weights
+        self._lora_touched = set()     # (owner, packed tensor) the merged set rewrote
+        self._pristine: Dict[tuple, torch.Tensor] = {}   # their pristine copies, made when a LoRA first touches one
+        self._lora_keys = None         # lora.KeyTable of this model, built on the first LoRA request
 
     @property
     def inpainting(self) -> bool:
@@ -555,7 +560,10 @@ class SDEngine:
         return self.plans[key]
 
     def release(self):
-        """drop every plan, graph and encoder program (factory.evict / LocalGPUWorker.restart)"""
+        """drop every plan, graph and encoder program (factory.evict / LocalGPUWorker.restart); merged LoRA networks are
+        taken out of the weights first and the pristine copies freed"""
+        self.set_loras(())
+        self._pristine.clear()
         for p in self.plans.values():
             p.graphs.clear()
         self.plans.clear()
@@ -563,6 +571,59 @@ class SDEngine:
         if self.device.type == "cuda":
             with self._ctx():
                 torch.cuda.empty_cache()
+
+    # ------------------------------------------------------------------------------------------ LoRA networks
+    def _lora_owners(self):
+        """{owner: (packed tensors, placements)}: the UNet and the text towers (ControlNets and the VAE are never touched)"""
+        towers = [("t0", self.clip.t0)] + ([("t1", self.clip.t1)] if self.clip.xl else [])
+        return {"unet": (self.unet_w.t, self.unet_w.place), **{n: (t.w, t.place) for n, t in towers}}
+
+    def lora_key_table(self) -> "L.KeyTable":
+        """sdwui's network_layer_mapping of this model: UNet names without `model.`, text towers without
+        `cond_stage_model.` (SD1.x, SD 2.x) or `conditioner.embedders.` (SDXL)"""
+        if self._lora_keys is None:
+            cut = "conditioner.embedders." if self.clip.xl else "cond_stage_model."
+            owners = [("unet", self.unet_w.place, UNET_PREFIX[:-len("diffusion_model.")], False)]
+            owners += [(n, pl, cut, True) for n, (_, pl) in self._lora_owners().items() if n != "unet"]
+            self._lora_keys = L.KeyTable(owners, self.unet_cfg, self.clip_cfg.open_clip)
+        return self._lora_keys
+
+    @torch.no_grad()
+    def set_loras(self, nets=()):
+        """Merge the LoRA networks `nets` [(lora.LoraFile, lora.LoraRef)] into the packed UNet and text-tower weights, in
+        place on this engine's stream (captured graphs stay valid); () restores the pristine weights.  The set merged now
+        costs nothing; another set rewrites, from the pristine copies, only the tensors the old or the new set touches.
+        A tensor's pristine copy is made the first time a network touches it (an engine without LoRA requests holds
+        none).  Every output is bitwise the same on every device (ops.lora_merge)."""
+        key = tuple((f.key or (f.name, id(f)), r.te, r.unet, r.dyn) for f, r in nets)
+        if key == self._lora_set:
+            return
+        owners = self._lora_owners()
+        packed = {n: t for n, (t, _) in owners.items()}
+        with self._ctx():
+            groups = L.plan(L.resolve(self.lora_key_table(), list(nets)) if nets else [],
+                            {n: pl for n, (_, pl) in owners.items()}, packed, self.device)
+            touched = set(groups)
+            for k in self._lora_touched - touched:
+                groups[k] = [L.Group(0, packed[k[0]][k[1]].shape[0])]
+            targets = []
+            for (owner, name), gs in groups.items():
+                w = packed[owner][name]
+                p = self._pristine.get((owner, name))
+                if p is None:
+                    p = self._pristine[(owner, name)] = w.clone()
+                for g in gs:
+                    u = g.U if g.U is not None else torch.zeros((g.hi - g.lo, 0), device=self.device)
+                    d = g.D if g.D is not None else torch.zeros((0, w.shape[1]), device=self.device)
+                    targets.append((w[g.lo:g.hi], p[g.lo:g.hi], u, d))
+            ops.lora_merge(targets)
+        self._lora_set, self._lora_touched = key, touched
+
+    def _use_loras(self, loras):
+        """a request's networks: None (a request without tags) restores pristine weights if a set is merged, else
+        nothing happens"""
+        if loras is not None or self._lora_set:
+            self.set_loras(loras or ())
 
     @torch.no_grad()
     def encode_prompts(self, tokens: torch.Tensor, width: int = 512, height: int = 512, zero_txt: bool = False,
@@ -1083,7 +1144,7 @@ class SDEngine:
                 inpainting_fill: int = 1, multipliers: Optional[torch.Tensor] = None,
                 neg_multipliers: Optional[torch.Tensor] = None, controls=None, tiling: bool = False,
                 image_mask: Optional[torch.Tensor] = None, inpainting_mask_weight: float = 1.0,
-                token_merging_ratio: float = 0.0, schedule=None) -> torch.Tensor:
+                token_merging_ratio: float = 0.0, schedule=None, loras=None) -> torch.Tensor:
         """img2img: VAE-encode the init images (posterior mean), noise them to t_enc, run the remaining part of the
         sampler's schedule, decode.  init_u8 uint8 [b, H, W, 3].  Returns uint8 [b, H, W, 3] on device.
         `latmask` fp32 [h * w] (b200sd.inpaint.prepare_mask): inpainting — the region with latmask 0 is held to the init
@@ -1105,8 +1166,11 @@ class SDEngine:
         merge.
         `schedule` = (cond PromptSchedule, uncond PromptSchedule): prompt editing / alternation (sdwui's prompt
         schedules over the sampler's total steps); tokens / neg_tokens then give only the batch size.  None: the
-        tokens for every step."""
+        tokens for every step.
+        `loras`: LoRA networks [(lora.LoraFile, lora.LoraRef)] merged for this request (set_loras); None: pristine
+        weights."""
         b = tokens.shape[0]
+        self._use_loras(loras)
         cond, uncond, sched = self._pass_conds(tokens, neg_tokens, init_u8.shape[2], init_u8.shape[1], multipliers,
                                                neg_multipliers, schedule)
         init = self.encode(init_u8, tiling)
@@ -1156,7 +1220,8 @@ class SDEngine:
                       neg_multipliers: Optional[torch.Tensor] = None, upscaler: str = "Latent",
                       upscaler_tile: int = 192, upscaler_overlap: int = 8, tiling: bool = False,
                       inpainting_mask_weight: float = 1.0, token_merging_ratio: float = 0.0,
-                      token_merging_ratio_hr: float = 0.0, schedule=None, hr_schedule=None) -> torch.Tensor:
+                      token_merging_ratio_hr: float = 0.0, schedule=None, hr_schedule=None, loras=None,
+                      hr_loras=None) -> torch.Tensor:
         """txt2img with sdwui's hires fix (StableDiffusionProcessingTxt2Img.sample / sample_hr_pass): first pass at
         (height, width), the `upscaler` to hr_scale x, a fresh per-image noise of the large shape from the same seeds,
         then the same sampler's img2img half from t_enc with `hr_steps` (0 = `steps`) steps, decode at the large size.
@@ -1171,6 +1236,8 @@ class SDEngine:
         `schedule` as for img2img, for the first pass; `hr_schedule` the second pass's own (sdwui hr_prompt /
         hr_negative_prompt over the hires steps, with the first pass's steps as the base of its offsets), required with
         `schedule`; without both the second pass takes the first pass's prompts.
+        `loras` as for img2img, for the first pass; `hr_loras` the second pass's own networks (sdwui
+        hr_extra_network_data; () for none), which re-encode its prompts; None: the first pass's.
         Returns uint8 [b, H*hr, W*hr, 3] on device."""
         from . import upscale
         if schedule is not None and hr_schedule is None:
@@ -1181,6 +1248,7 @@ class SDEngine:
             raise ValueError(f"hires upscaler {upscaler!r} with inpainting_mask_weight {inpainting_mask_weight} < 1 is not "
                              f"served on an inpainting model")
         b = tokens.shape[0]
+        self._use_loras(loras)
         h, w = height // 8, width // 8
         h2, w2 = int(height * hr_scale) // 8, int(width * hr_scale) // 8
         if kind != "latent" and (int(height * hr_scale) % 8 or int(width * hr_scale) % 8):
@@ -1208,9 +1276,11 @@ class SDEngine:
             init = self.encode(images.contiguous(), tiling)
             if self.inpainting:
                 image_cond = (self.encode_conditioning(images.contiguous(), None, inpainting_mask_weight, tiling), None)
+        if hr_loras is not None:
+            self.set_loras(hr_loras)
         if hr_schedule is not None:
             cond, uncond, sched = self._pass_conds(tokens, neg_tokens, w2 * 8, h2 * 8, None, None, hr_schedule)
-        elif self.clip.xl:   # SDXL's vector conditioning carries the target size: the second pass gets its own (sdwui hr_c / hr_uc)
+        elif self.clip.xl or hr_loras is not None:   # SDXL's vector conditioning carries the target size: the second pass gets its own (sdwui hr_c / hr_uc)
             cond, uncond, sched = self._pass_conds(tokens, neg_tokens, w2 * 8, h2 * 8, multipliers, neg_multipliers,
                                                    schedule)
         lat2 = self._sample_from(init, cond, uncond, seed, denoising_strength, hr_steps or steps, cfg_scale, sampler, scheduler,
@@ -1232,13 +1302,14 @@ class SDEngine:
                 height: int = 512, width: int = 512, sampler: str = "DDIM", scheduler: Optional[str] = None,
                 multipliers: Optional[torch.Tensor] = None, neg_multipliers: Optional[torch.Tensor] = None,
                 controls=None, tiling: bool = False, inpainting_mask_weight: float = 1.0,
-                token_merging_ratio: float = 0.0, schedule=None) -> torch.Tensor:
+                token_merging_ratio: float = 0.0, schedule=None, loras=None) -> torch.Tensor:
         """Whole request for this engine's share: returns uint8 [b, H, W, 3] on device.  tokens [b, 77 * k] and
         neg_tokens [b, 77 * k'] with their optional emphasis multipliers of the same shapes (factory.tokenize_prompts).
         `controls`: ControlNet units as for img2img (None: none); `tiling` as for img2img.  An inpainting model gets
         sdwui's txt2img conditioning, which inpainting_mask_weight does not enter (it is taken for a uniform call).
-        `token_merging_ratio` and `schedule` as for img2img."""
+        `token_merging_ratio`, `schedule` and `loras` as for img2img."""
         b = tokens.shape[0]
+        self._use_loras(loras)
         h, w = height // 8, width // 8
         cond, uncond, sched = self._pass_conds(tokens, neg_tokens, width, height, multipliers, neg_multipliers, schedule)
         lat = self._sample_txt(cond, uncond, seed, b, h, w, steps, cfg_scale, sampler, scheduler, controls, tiling,

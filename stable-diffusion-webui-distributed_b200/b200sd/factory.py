@@ -7,6 +7,7 @@ a 9-channel UNet (`sd15-inpainting`, ...).  A checkpoint's own conv_in decides b
 checkpoint serves it as one.  Prediction type: each family's default (v for sd21 / tiny21, eps for the others and for
 every inpainting model, as sdwui's v2-inpainting-inference.yaml), overridden by B200SD_PREDICTION = eps | v.
 ControlNets (controlnet()): B200SD_CONTROLNET_DIR/<model>.safetensors, otherwise seeded synthetic weights.
+LoRA networks (loras()): B200SD_LORA_DIR/<name>.safetensors (kohya format), otherwise a seeded synthetic LoRA.
 """
 import dataclasses
 import logging
@@ -20,7 +21,8 @@ import torch
 
 from . import config as C
 from .engine import SDEngine
-from .synth import make_controlnet_state_dict, make_state_dict
+from . import lora as L
+from .synth import make_controlnet_state_dict, make_lora_state_dict, make_state_dict
 from .unet_exec import ControlNetWeights
 
 log = logging.getLogger("distributed")
@@ -167,6 +169,62 @@ def controlnet(name: str, size: str = None, device: str = "cuda:0", dtype=torch.
         for k in mine[:max(0, len(mine) - MAX_CONTROLNETS)]:
             del _CONTROLNETS[k]
     return cw
+
+
+MAX_LORAS = 8   # parsed LoRA files kept per process; the least recently used one is dropped beyond that
+_LORAS: "OrderedDict[tuple, L.LoraFile]" = OrderedDict()
+
+
+def lora_file(name: str, unet_cfg: C.UNetConfig, clip_cfg: C.CLIPConfig) -> Optional[L.LoraFile]:
+    """LoRA `name` parsed (lora.load_state_dict: ValueError for a network type that is not served) and cached under
+    (path, size, mtime): B200SD_LORA_DIR/<name>.safetensors, None with a warning when the variable is set and the file is
+    missing (sdwui's "Networks not found"), or a seeded synthetic LoRA for the model of (unet_cfg, clip_cfg) (crc32 of
+    the name) when it is not set"""
+    root = os.environ.get("B200SD_LORA_DIR")
+    if not root:
+        log.warning("b200sd: B200SD_LORA_DIR is not set — LoRA %r is a SEEDED SYNTHETIC network; set it to a directory "
+                    "of <name>.safetensors files for real ones", name)
+        key = ("synthetic", unet_cfg, clip_cfg, name)
+    else:
+        path = os.path.join(root, name + ".safetensors")
+        if not os.path.isfile(path):
+            log.warning("b200sd: Networks not found: %s (no %s)", name, path)
+            return None
+        st = os.stat(path)
+        key = (path, st.st_size, st.st_mtime_ns)
+    with _LOCK:
+        f = _LORAS.get(key)
+        if f is not None:
+            _LORAS.move_to_end(key)
+            return f
+    if not root:
+        sd = make_lora_state_dict(unet_cfg, clip_cfg, seed=zlib.crc32(name.encode("utf-8")),
+                                  form="compvis" if clip_cfg.xl_width else "diffusers")
+    else:
+        sd = _load_safetensors(key[0])
+    f = L.load_state_dict(name, sd, key)
+    with _LOCK:
+        _LORAS[key] = f
+        while len(_LORAS) > MAX_LORAS:
+            _LORAS.popitem(last=False)
+    return f
+
+
+def loras(refs, eng) -> List[tuple]:
+    """prompt tags (lora.LoraRef) -> [(LoraFile, LoraRef)] for the SDEngine `eng`; missing files are skipped with a
+    warning.  Every file is read (and refused if need be) before the engine changes any weight."""
+    out = []
+    for ref in refs:
+        f = lora_file(ref.name, eng.unet_cfg, eng.clip_cfg)
+        if f is not None:
+            out.append((f, ref))
+    return out
+
+
+def refresh_loras():
+    """forget the parsed LoRA files (refresh-loras): the next request reads them again"""
+    with _LOCK:
+        _LORAS.clear()
 
 
 def model_identity(size: str = None) -> str:

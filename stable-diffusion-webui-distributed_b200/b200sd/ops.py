@@ -644,3 +644,30 @@ def tome_unmerge_add(residual: torch.Tensor, y: torch.Tensor, slot: torch.Tensor
     check(rc, f"b200sd_tome_unmerge_add NB={nb} N={n} Nm={nm} C={c}")
     _count()
     return out
+
+
+def lora_merge(targets):
+    """targets: [(W, P, U, D)] — W / P fp16 or bf16 views [rows, cols] with contiguous rows and one row pitch, U fp32
+    [rows, R], D fp32 [R, cols] (R = 0: U [rows, 0], a restore).  Every W = round(P + U @ D) in ONE launch
+    (b200sd_lora_merge; the descriptor table is copied to the device first).  The tensors must stay allocated until the
+    launch has run on the current stream (torch's allocator reuses them in stream order only)."""
+    if not targets:
+        return None
+    table = (_lib.LoraTarget * len(targets))()
+    dt = None
+    for i, (w, p, u, d) in enumerate(targets):
+        rows, cols = w.shape
+        r = u.shape[1]
+        assert p.shape == w.shape and p.stride() == w.stride() and w.stride(1) == 1 and p.dtype == w.dtype
+        assert u.dtype == torch.float32 and d.dtype == torch.float32 and u.is_contiguous() and d.is_contiguous()
+        assert tuple(u.shape) == (rows, r) and tuple(d.shape) == (r, cols)
+        dt = _dt(w) if dt is None else dt
+        assert _dt(w) == dt, "one dtype per launch"
+        table[i] = _lib.LoraTarget(w.data_ptr(), p.data_ptr(), u.data_ptr() if r else 0, d.data_ptr() if r else 0,
+                                   w.stride(0), rows, cols, r, 0)
+    dev = targets[0][0].device
+    buf = torch.frombuffer(bytearray(bytes(table)), dtype=torch.uint8).to(dev)
+    rc = _lib.lib().b200sd_lora_merge(_p(buf), len(targets), dt, _stream())
+    check(rc, f"b200sd_lora_merge targets={len(targets)}")
+    _count()
+    return buf

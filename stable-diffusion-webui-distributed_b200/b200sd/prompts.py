@@ -16,8 +16,10 @@ parses with lark's Earley parser, which resolves the ambiguity between a group a
 colon characters right after its closer in a way that depends on the rest of the prompt (`x [b:c:4]]] y` and
 `[a:b:5]):` stay literal text there, `[a:1]:` does not); prompt_schedule always parses such a group.
 
-Not interpreted (as text they reach the tokenizer unchanged): composable `AND`, textual-inversion embeddings and
-extra-network tags.
+Extra-network tags (`<lora:name:0.8>`, sdwui extra_networks.parse_prompt) are cut out of the positive prompt before any
+of this by b200sd.lora.parse_prompt, which also turns lora / lyco tags into the networks merged for the request.
+
+Not interpreted (as text they reach the tokenizer unchanged): composable `AND` and textual-inversion embeddings.
 """
 import re
 from typing import Callable, List, Optional, Sequence, Tuple

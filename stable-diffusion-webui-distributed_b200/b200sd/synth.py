@@ -223,3 +223,105 @@ def make_state_dict(unet: UNetConfig, vae: VAEConfig, clip: CLIPConfig, seed: in
     else:
         _clip(i, clip)
     return i.sd
+
+
+def _lora_unet_modules(cfg: UNetConfig):
+    """(ldm module path, kind, out, in) of every UNet layer a kohya LoRA trains: kind "conv3" (LoCon 3x3), "conv1"
+    (1x1 conv) or "linear"
+    """
+    ted = cfg.time_embed_dim
+    mods = [("time_embed.0", "linear", ted, cfg.model_channels), ("time_embed.2", "linear", ted, ted)]
+    if cfg.adm_in_channels:
+        mods += [("label_emb.0.0", "linear", ted, cfg.adm_in_channels), ("label_emb.0.2", "linear", ted, ted)]
+    proj = "linear" if cfg.linear_proj else "conv1"
+    inputs, middle, outputs = unet_layout(cfg)
+    for prefix, blocks in [("input_blocks", inputs), ("middle_block", [middle]), ("output_blocks", outputs)]:
+        for n, layers in enumerate(blocks):
+            for j, layer in enumerate(layers):
+                key = f"{prefix}.{n}.{j}" if prefix != "middle_block" else f"middle_block.{j}"
+                if layer[0] == "conv_in":
+                    mods.append((key, "conv3", layer[2], layer[1]))
+                elif layer[0] == "res":
+                    cin, cout = layer[1], layer[2]
+                    mods += [(key + ".in_layers.2", "conv3", cout, cin), (key + ".out_layers.3", "conv3", cout, cout),
+                             (key + ".emb_layers.1", "linear", cout, ted)]
+                    if cin != cout:
+                        mods.append((key + ".skip_connection", "conv1", cout, cin))
+                elif layer[0] == "attn":
+                    c = layer[1]
+                    mods += [(key + ".proj_in", proj, c, c), (key + ".proj_out", proj, c, c)]
+                    for d in range(layer[2]):
+                        t = f"{key}.transformer_blocks.{d}"
+                        for a, ctx in (("attn1", c), ("attn2", cfg.context_dim)):
+                            mods += [(f"{t}.{a}.to_q", "linear", c, c), (f"{t}.{a}.to_k", "linear", c, ctx),
+                                     (f"{t}.{a}.to_v", "linear", c, ctx), (f"{t}.{a}.to_out.0", "linear", c, c)]
+                        mods += [(f"{t}.ff.net.0.proj", "linear", 8 * c, c), (f"{t}.ff.net.2", "linear", c, 4 * c)]
+                elif layer[0] == "down":
+                    mods.append((key + ".op", "conv3", layer[1], layer[1]))
+                elif layer[0] == "up":
+                    mods.append((key + ".conv", "conv3", layer[1], layer[1]))
+    mods.append(("out.2", "conv3", cfg.out_channels, cfg.model_channels))
+    return mods
+
+
+def _diffusers_name(path: str, blocks: Dict[str, str]) -> str:
+    """kohya's diffusers-form module name of an ldm UNet module path (inverse of lora.to_compvis)"""
+    flat = path.replace(".", "_")
+    if flat == "input_blocks_0_0":
+        return "lora_unet_conv_in"
+    if flat == "out_2":
+        return "lora_unet_conv_out"
+    if flat.startswith("time_embed_"):
+        return f"lora_unet_time_embedding_linear_{int(flat[len('time_embed_'):]) // 2 + 1}"
+    inverse = {"in_layers_2": "conv1", "out_layers_3": "conv2", "emb_layers_1": "time_emb_proj",
+               "skip_connection": "conv_shortcut"}
+    for diff, ldm in sorted(blocks.items(), key=lambda kv: -len(kv[1])):
+        if flat.startswith(ldm + "_"):
+            suffix = flat[len(ldm) + 1:]
+            if "_resnets_" in diff:
+                suffix = inverse.get(suffix, suffix)
+            elif "_downsamplers_" in diff and suffix == "op":
+                suffix = "conv"
+            return f"lora_unet_{diff}_{suffix}"
+    return "lora_unet_" + flat   # no diffusers name (SDXL's label_emb): the compvis form
+
+
+def make_lora_state_dict(unet: UNetConfig, clip: CLIPConfig, seed: int = 0, rank: int = 8, form: str = "diffusers",
+                         unet_modules: bool = True, te_modules: bool = True) -> Dict[str, torch.Tensor]:
+    """A seeded kohya-format LoRA (LoCon) for the model of (unet, clip): `<module>.lora_down.weight`,
+    `.lora_up.weight`, `.alpha` (rank / 2) for every UNet linear / conv layer (3x3 convs as LoCon: down [r, Cin, 3, 3],
+    up [Cout, r, 1, 1]) and every text-tower attention / MLP linear, under kohya's names: `lora_unet_` in the diffusers
+    form (`down_blocks_0_resnets_1_conv1`, ...) or the compvis form (`input_blocks_1_0_in_layers_2`, ...; SDXL files use
+    it), `lora_te_` (SD1.x, SD 2.x), `lora_te1_` / `lora_te2_` (SDXL) with HF CLIP layer names.  Each delta is about 15 %
+    of its weight at multiplier 1."""
+    from .lora import diffusers_blocks
+    if form not in ("diffusers", "compvis"):
+        raise ValueError(form)
+    g = torch.Generator(device="cpu").manual_seed(seed)
+    sd: Dict[str, torch.Tensor] = {}
+
+    def add(name, kind, cout, cin):
+        k = 3 if kind == "conv3" else 1
+        conv = kind != "linear"
+        down = torch.randn((rank, cin * k * k), generator=g) / math.sqrt(cin * k * k)
+        up = torch.randn((cout, rank), generator=g) * (0.3 / math.sqrt(rank))
+        sd[name + ".lora_down.weight"] = down.reshape(rank, cin, k, k) if conv else down
+        sd[name + ".lora_up.weight"] = up.reshape(cout, rank, 1, 1) if conv else up
+        sd[name + ".alpha"] = torch.tensor(rank / 2.0)
+
+    if unet_modules:
+        blocks = diffusers_blocks(unet)
+        for path, kind, cout, cin in _lora_unet_modules(unet):
+            add(_diffusers_name(path, blocks) if form == "diffusers" else "lora_unet_" + path.replace(".", "_"),
+                kind, cout, cin)
+    if te_modules:
+        towers = [("lora_te1_", clip.width, clip.layers), ("lora_te2_", clip.xl_width, clip.xl_layers)] if clip.xl_width \
+            else [("lora_te_", clip.width, clip.layers)]
+        for prefix, w, layers in towers:
+            for l in range(layers):
+                p = f"{prefix}text_model_encoder_layers_{l}_"
+                for n in ("q_proj", "k_proj", "v_proj", "out_proj"):
+                    add(p + "self_attn_" + n, "linear", w, w)
+                add(p + "mlp_fc1", "linear", 4 * w, w)
+                add(p + "mlp_fc2", "linear", w, 4 * w)
+    return sd

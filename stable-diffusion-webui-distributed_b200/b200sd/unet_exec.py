@@ -23,7 +23,7 @@ import torch
 
 from . import ops
 from .config import CONTROL_PREFIX, UNET_PREFIX, UNetConfig, controlnet_layout, unet_layout
-from .weights import pack_conv, pack_geglu, pad_heads
+from .weights import Placement, conv_columns, index_column, pack_conv, pack_geglu, pad_heads, source_rows
 
 
 MAX_CONTROLS = 3   # ControlNet units per request (sd-webui-controlnet's default unit count)
@@ -74,6 +74,7 @@ class UNetWeights:
         self.layout = unet_layout(cfg)
         self.res_keys: List[str] = []     # every ResBlock in execution order
         self.res_off: Dict[str, int] = {}  # offset of its conv1 bias inside the per-step bias row
+        self.place: Dict[str, Placement] = {}   # ldm weight key -> where it lies in self.t (b200sd/lora.py)
         self._pack()
 
     # -- helpers
@@ -87,7 +88,9 @@ class UNetWeights:
         return self._dev(self._w(key), torch.float32)
 
     def _conv(self, name, key, cin_pad=0, cout_pad=0):
-        self.t[name + ".w"] = self._dev(pack_conv(self._w(key + ".weight"), cin_pad, cout_pad))
+        w = self._w(key + ".weight")
+        self.t[name + ".w"] = self._dev(pack_conv(w, cin_pad, cout_pad))
+        self.place[self.p + key + ".weight"] = Placement(name + ".w", tuple(w.shape), None, conv_columns(w.shape, cin_pad))
         b = self._w(key + ".bias")
         if cout_pad > b.numel():
             b = torch.cat([b, b.new_zeros(cout_pad - b.numel())])
@@ -96,6 +99,7 @@ class UNetWeights:
     def _lin(self, name, key, bias=True):
         w = self._w(key + ".weight")
         self.t[name + ".w"] = self._dev(w.reshape(w.shape[0], -1))
+        self.place[self.p + key + ".weight"] = Placement(name + ".w", tuple(w.shape))
         if bias:
             self.t[name + ".b"] = self._f32(key + ".bias")
 
@@ -123,6 +127,8 @@ class UNetWeights:
             if cin != cout:
                 self._lin(key + ".skip", key + ".skip_connection")
             emb_w.append(self._w(key + ".emb_layers.1.weight"))
+            self.place[self.p + key + ".emb_layers.1.weight"] = Placement("emb_all.w", (cout, cfg.time_embed_dim),
+                                                                          torch.arange(cout) + off)
             emb_b.append(self._w(key + ".emb_layers.1.bias"))
             conv1_b.append(self._w(key + ".in_layers.2.bias"))
             self.res_keys.append(key)
@@ -136,12 +142,16 @@ class UNetWeights:
             self._norm(key + ".norm", key + ".norm")
             self._lin(key + ".proj_in", key + ".proj_in")    # conv 1x1 (SD1.x) and Linear (SDXL) are the same GEMM in NHWC
             self._lin(key + ".proj_out", key + ".proj_out")
+            head_rows = source_rows(pad_heads(index_column(c), heads, d, dp))
             for i in range(depth):
                 t = f"{key}.transformer_blocks.{i}"
                 for n in ("norm1", "norm2", "norm3"):
                     self._norm(f"{t}.{n}", f"{t}.{n}")
                 qkv = torch.cat([pad_heads(self._w(f"{t}.attn1.to_{n}.weight"), heads, d, dp) for n in "qkv"])
                 self.t[f"{t}.attn1.qkv.w"] = self._dev(qkv)
+                for j, n in enumerate("qkv"):
+                    self.place[f"{self.p}{t}.attn1.to_{n}.weight"] = Placement(f"{t}.attn1.qkv.w", (c, c),
+                                                                                head_rows + j * heads * dp)
                 # V's first pad column of every head is driven to exactly 1 through the bias: the P.V MMA then
                 # returns the softmax denominators in accumulator column d (b200sd_attention v_ones_col)
                 ones = torch.zeros((heads, dp))
@@ -153,13 +163,20 @@ class UNetWeights:
                                                       torch.float32)
                 self._lin(f"{t}.attn1.out", f"{t}.attn1.to_out.0")
                 self.t[f"{t}.attn2.q.w"] = self._dev(pad_heads(self._w(f"{t}.attn2.to_q.weight"), heads, d, dp))
+                self.place[f"{self.p}{t}.attn2.to_q.weight"] = Placement(f"{t}.attn2.q.w", (c, c), head_rows)
                 kv = torch.cat([pad_heads(self._w(f"{t}.attn2.to_{n}.weight"), heads, d, dp) for n in "kv"])
                 self.t[f"{t}.attn2.kv.w"] = self._dev(kv)
+                for j, n in enumerate("kv"):
+                    self.place[f"{self.p}{t}.attn2.to_{n}.weight"] = Placement(f"{t}.attn2.kv.w", (c, cfg.context_dim),
+                                                                              head_rows + j * heads * dp)
                 self._lin(f"{t}.attn2.out", f"{t}.attn2.to_out.0")
                 w, b = self._w(f"{t}.ff.net.0.proj.weight"), self._w(f"{t}.ff.net.0.proj.bias")
                 bn = ops.pick_block_n(w.shape[0], geglu=True)
                 wp, bp = pack_geglu(w, b, bn)
                 self.t[f"{t}.ff1.w"] = self._dev(wp)
+                idx = index_column(w.shape[0])
+                self.place[f"{self.p}{t}.ff.net.0.proj.weight"] = Placement(
+                    f"{t}.ff1.w", tuple(w.shape), source_rows(pack_geglu(idx, idx[:, 0], bn)[0]))
                 self.t[f"{t}.ff1.b"] = self._dev(bp, torch.float32)
                 self._lin(f"{t}.ff2", f"{t}.ff.net.2")
 

@@ -4,8 +4,47 @@ Upstream (ldm) layouts -> kernel layouts:
   conv  [Cout, Cin, kh, kw]        -> [Cout, kh*kw*Cin]  (tap-major, channels innermost: matches NHWC im2col order)
   GEGLU proj [2*inner, C] (+bias)  -> rows interleaved per output tile: [value half | gate half] per block_n rows
   q/k/v projections [h*d, C]       -> [h*d_pad, C] with zero rows for the padded head columns
+
+Every packer also records, per ldm weight key, a Placement: where each source row and column landed.  LoRA merging
+(b200sd/lora.py) scatters its factors through these, so the layouts are known here only.  They are found by running the
+packers themselves on index tensors (value = source index + 1, 0 = padding).
 """
+from dataclasses import dataclass
+from typing import Optional
+
 import torch
+
+
+@dataclass
+class Placement:
+    """an ldm weight of `shape` [out, in...] inside a packed tensor: tensor name in its owner's dict, the packed row of
+    every source row (None: row i -> row i) and the source column (flattened [Cin, kh, kw]) of every packed column (-1:
+    padding; None: identity)"""
+    tensor: str
+    shape: tuple
+    rows: Optional[torch.Tensor] = None
+    cols: Optional[torch.Tensor] = None
+
+
+def index_column(n: int) -> torch.Tensor:
+    """[n, 1] float64 with value i + 1 in row i: a weight whose packing shows where each row goes"""
+    return (torch.arange(n, dtype=torch.float64) + 1)[:, None]
+
+
+def source_rows(packed: torch.Tensor) -> torch.Tensor:
+    """packed [R', 1] (an index_column through a packer) -> int64 [n]: the packed row of each source row"""
+    v = packed[:, 0].long() - 1
+    pos = torch.nonzero(v >= 0)[:, 0]
+    out = torch.empty(int(v.max()) + 1, dtype=torch.long)
+    out[v[pos]] = pos
+    return out
+
+
+def conv_columns(shape, cin_pad: int = 0) -> torch.Tensor:
+    """source column of every packed column of pack_conv(w [Cout, Cin, kh, kw], cin_pad) (-1: padded channel)"""
+    _, cin, kh, kw = shape
+    idx = (torch.arange(cin * kh * kw, dtype=torch.float64) + 1).reshape(1, cin, kh, kw)
+    return pack_conv(idx, cin_pad)[0].long() - 1
 
 
 def pack_conv(w: torch.Tensor, cin_pad: int = 0, cout_pad: int = 0) -> torch.Tensor:

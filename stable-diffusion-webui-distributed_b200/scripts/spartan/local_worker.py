@@ -79,7 +79,9 @@ class LocalGPUWorker(Worker):
         self.set_state(State.INTERRUPTED)
 
     def refresh_checkpoints(self):
-        return None
+        """the reference posts refresh-checkpoints and refresh-loras: LoRA files are read again on their next use"""
+        from b200sd import factory
+        factory.refresh_loras()
 
     def available_models(self):
         return []
@@ -218,27 +220,37 @@ class LocalGPUWorker(Worker):
             subseed = random.randrange(4294967294)
         cfg_scale = float(payload.get("cfg_scale", 7.0))
         strength = float(payload.get("subseed_strength") or 0.0)
+        # sdwui extra networks: the tags leave the positive prompts before scheduling and tokenization (the infotext keeps
+        # them); every named LoRA file is read, and refused if need be, before the engine changes a weight
+        from b200sd import factory, lora
+        body, refs = lora.parse_prompt(prompt)
+        nets = factory.loras(refs, eng) if refs else []
+        hires_fix = bool(payload.get("enable_hr")) and not payload.get("init_images")
+        hr_body, hr_nets = body, nets
+        if hires_fix and payload.get("hr_prompt"):   # sdwui hr_extra_network_data: hr_prompt's own tags
+            hr_body, hr_refs = lora.parse_prompt(payload["hr_prompt"])
+            hr_nets = factory.loras(hr_refs, eng) if hr_refs else []
         vocab = eng.clip_cfg.vocab
         pad = getattr(eng.clip_cfg, "pad_id", None)   # the token after each chunk's first EOS (SD 2.x: 0)
         mult_all = None
         # prompt editing / alternation: sdwui's schedules over the sampler's total steps.  A prompt whose schedule has
         # one entry is that entry's text (the prompt itself without schedule syntax) for every step.
         sched_kw, hr_kw = {}, {}
-        cond_text, neg_text = prompt, negative
+        cond_text, neg_text = body, negative
         if "prompt_tokens" not in payload:
             from b200sd.engine import total_steps
             old = self._use_old_scheduling(payload)
             base = total_steps(sampler, steps)
-            cs = self._schedule(prompt, base, None, old, vocab, pad)
+            cs = self._schedule(body, base, None, old, vocab, pad)
             us = self._schedule(negative, base, None, old, vocab, pad)
             if len(cs[0].ends) > 1 or len(us[0].ends) > 1:
                 sched_kw["schedule"] = (cs[0], us[0])
             cond_text, neg_text = cs[1][0], us[1][0]
-            if payload.get("enable_hr") and not payload.get("init_images"):
+            if hires_fix:
                 # sdwui calculate_hr_conds: hr_prompt / hr_negative_prompt (empty: the first pass's), over the hires
                 # steps with the first pass's as the base of the offsets
                 hires = total_steps(sampler, int(payload.get("hr_second_pass_steps") or 0) or steps)
-                hc = self._schedule(payload.get("hr_prompt") or prompt, base, hires, old, vocab, pad)
+                hc = self._schedule(hr_body, base, hires, old, vocab, pad)
                 hu = self._schedule(payload.get("hr_negative_prompt") or negative, base, hires, old, vocab, pad)
                 if sched_kw or len(hc[1]) > 1 or len(hu[1]) > 1 or (hc[1][0], hu[1][0]) != (cond_text, neg_text):
                     hr_kw["hr_schedule"] = (hc[0], hu[0])
@@ -258,6 +270,8 @@ class LocalGPUWorker(Worker):
             weights["tiling"] = True
         if mask_weight is not None:
             weights["inpainting_mask_weight"] = mask_weight
+        if nets:       # likewise a payload without LoRA tags
+            weights["loras"] = nets
         tome, tome_hr = self._token_merging(payload, img2img=init_u8 is not None)
         # a payload whose ratio resolves to 0 (or below: nothing is merged) reaches the engine with exactly the
         # arguments it always had
@@ -283,6 +297,9 @@ class LocalGPUWorker(Worker):
                 if payload.get("hr_resize_x") and payload.get("hr_resize_y"):
                     hr_scale = float(payload["hr_resize_x"]) / width
                 hires = dict(weights, **tome_kw, **hr_kw)
+                same = lambda a, b: [(f.key, r) for f, r in a] == [(f.key, r) for f, r in b]  # noqa: E731
+                if not same(hr_nets, nets):   # the second pass's own networks (none: pristine weights)
+                    hires["hr_loras"] = hr_nets
                 if tome_hr > 0:
                     hires["token_merging_ratio_hr"] = float(tome_hr)
                 hires.update(self._hires_upscaler(payload, width, height, hr_scale))

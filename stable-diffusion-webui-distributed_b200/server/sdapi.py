@@ -180,6 +180,8 @@ def create_app(engine_factory: Callable, devices: Optional[List[int]] = None, ap
 
     @app.post(f"{API}/refresh-loras", dependencies=[Depends(auth)])
     def refresh_loras():
+        from b200sd import factory
+        factory.refresh_loras()
         return None
 
     @app.get(f"{API}/sd-models", dependencies=[Depends(auth)])
